@@ -37,7 +37,7 @@ int tn_set_sm_margin(int sms);
 /* Tuning knob: raster group of the GEMM = number of 128-row M blocks whose tiles are walked across all N blocks before
  * moving on (default 8; decides which operand strips stay L2-resident between waves).  Results do not depend on it. */
 int tn_set_gemm_group(int m_blocks);
-int tn_set_gemm_split_tail(int on);  /* accepted for API compatibility; the 128x128-tile GEMM has no half-tile tail mode */
+int tn_set_gemm_split_tail(int on);  /* accepted for API compatibility; the GEMM has no half-tile tail mode */
 int tn_set_gemm_l2_hints(int on);   /* 1: A strips evict-last, B strips evict-first in the GEMM's TMA loads (default 0) */
 
 /* ---------------------------------------------------------------------------------------------------------------

@@ -6,14 +6,17 @@
 // and their autograd backward (dgrad, wgrad).
 //
 // Design (H100, one CTA per SM, persistent, warp-specialised):
-//   warpgroup 0     : TMA producer - one thread streams 128 x 64 A and B tiles (128B swizzle) into a STAGES-deep
+//   warpgroup 0     : TMA producer - one thread streams 128 x 64 A and BN x 64 B tiles (128B swizzle) into a STAGES-deep
 //                     shared-memory ring guarded by full / empty mbarriers; it runs ahead into the next tile while the
-//                     consumers are still in the epilogue of the current one
-//   warpgroups 1, 2 : consumers - each issues wgmma.m64n128k16 on its 64 rows of the 128 x 128 tile (fp32 accumulator in
-//                     registers), then runs the epilogue straight from registers to global memory
-// Operands may be K-major or MN-major (the transpose bits of wgmma), so forward, dgrad and wgrad all run on the
-// tensors where they lie: no transposes, no copies.  Epilogues: D = acc (+R) in bf16 or fp32, SwiGLU (gate and up
-// halves of one tile), SwiGLU backward on the dH accumulator, RoPE on the q/k columns of the fused QKV projection.
+//                     consumers are still in the epilogue of the current one.  setmaxnreg gives its registers away.
+//   warpgroups 1, 2 : consumers - each issues wgmma.m64n{BN}k16 on its 64 rows of the 128 x BN tile (fp32 accumulator in
+//                     registers), then writes the finished values into 64-row swizzled staging sub-tiles in shared memory
+//                     that TMA stores push to global memory; the stores drain while the next tile's MMAs run
+// BN = 256 (m64n256: half the shared-memory operand traffic per FLOP of the 128-wide tile) or 128, chosen on the host from
+// the wave count of the shape (pick_bn).  Operands may be K-major or MN-major (the transpose bits of wgmma), so
+// forward, dgrad and wgrad all run on the tensors where they lie: no transposes, no copies.  Epilogues: D = acc (+R) in
+// bf16 or fp32, SwiGLU (gate and up halves of one tile), SwiGLU backward on the dH accumulator, RoPE on the q/k columns of
+// the fused QKV projection.  Each output element sums its k-blocks in the same order at either tile width.
 #include <stdio.h>
 #include <stdlib.h>
 
@@ -24,16 +27,21 @@
 namespace tn {
 
 constexpr int BM = 128;
-constexpr int BN = 128;   // accumulator columns per tile (SwiGLU: 64 gate + 64 up)
 constexpr int BK = 64;
-constexpr int STAGES = 5;
 constexpr int GEMM_THREADS = 384;
 constexpr int A_BYTES = BM * BK * 2;              // 16 KB
-constexpr int B_BYTES = BN * BK * 2;              // 16 KB
-constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-constexpr int GEMM_SMEM = STAGES * STAGE_BYTES + 256 + 1024;   // + barriers + alignment slack
+constexpr int SUB_BYTES = 64 * 128;               // one staging sub-tile: 64 rows x 128 B (64 bf16 or 32 fp32 columns)
+constexpr int STAGING_BYTES = 2 * 2 * SUB_BYTES;  // two sub-tile buffers per consumer warpgroup
+constexpr int SMEM_LIMIT = 227 * 1024;
+template <int BN>
+struct TileCfg {
+  static constexpr int B_BYTES = BN * BK * 2;     // 16 KB (BN 128) / 32 KB (BN 256)
+  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+  static constexpr int STAGES = (SMEM_LIMIT - STAGING_BYTES - 256 - 1024) / STAGE_BYTES;   // 6 / 4
+  static constexpr int SMEM = STAGES * STAGE_BYTES + STAGING_BYTES + 256 + 1024;          // + barriers + alignment slack
+};
 
-// EPI: 0 = bf16 D = acc (+R);  1 = SwiGLU (cols [0,64) gate, [64,128) up -> G, U, H);  2 = fp32 D = acc (+R);
+// EPI: 0 = bf16 D = acc (+R);  1 = SwiGLU (cols [0,BN/2) gate, [BN/2,BN) up -> G, U, H);  2 = fp32 D = acc (+R);
 //      3 = SwiGLU backward on the dH accumulator: dG = (dH*U) * silu'(G), dU = dH * silu(G)  (same rounding points as
 //          tn_swiglu_bwd_bf16 applied to the bf16-rounded dH, so the fused and the two-kernel paths agree bit for bit)
 struct GemmParams {
@@ -41,12 +49,9 @@ struct GemmParams {
   int num_m, num_n, num_k;
   int group;                 // raster: tiles walk `group` M blocks x all N blocks before moving down (L2 reuse of A)
   uint64_t hint_a, hint_b;   // L2 policy of the operand loads (tn_set_gemm_l2_hints)
-  void* D[3];                // D[0]: output (EPI 1: H; EPI 3: dG), D[1]: EPI 3 dU; d_seg: one tensor per row segment
-  int64_t ldd;
-  const void* R;
+  const void* R;             // residual, read in the accumulator layout (may alias the output: in-place accumulation)
   int64_t ldr;
-  bf16* G;                   // EPI 1 (optional)
-  bf16* U;
+  int has_g, has_u;          // EPI 1: G / U are written too
   // segmented operands: several weight tensors that are separate nn.Parameters (q/k/v projections) behave as one GEMM
   //   b_seg 1: B = [B0;B1;B2] stacked along N (fused QKV forward)       -> D columns [0,off1) [off1,off2) [off2,N)
   //   b_seg 2: B = [B0;B1;B2] stacked along K (fused QKV dgrad)         -> A columns ...
@@ -65,6 +70,12 @@ struct GemmParams {
   int64_t ld_gu;
 };
 
+// Operand and output tensor maps.  d[]: EPI 0/2 the output (d_seg: one map per segment), EPI 1 H / G / U, EPI 3 dG / dU;
+// output boxes are one staging sub-tile (64 rows x 128 B, 128B swizzle).
+struct GemmMaps {
+  CUtensorMap a, b[3], d[3];
+};
+
 __device__ __forceinline__ void decode_tile(int tile, int num_m, int num_n, int group, int& m_blk, int& n_blk) {
   const int per_group = group * num_n;
   const int g = tile / per_group;
@@ -75,28 +86,25 @@ __device__ __forceinline__ void decode_tile(int tile, int num_m, int num_n, int 
   n_blk = r / gsize;
 }
 
-__device__ __forceinline__ void st_bf16x2(bf16* p, int col, int N, float lo, float hi) {
-  if (col + 1 < N) *reinterpret_cast<uint32_t*>(p) = pack_bf16x2(lo, hi);
-  else if (col < N) *p = __float2bfloat16_rn(lo);
-}
-
-template <bool A_MN, bool B_MN, int EPI>
+template <int BN, bool A_MN, bool B_MN, int EPI>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB0,
-            const __grid_constant__ CUtensorMap tmB1, const __grid_constant__ CUtensorMap tmB2, const GemmParams p) {
+gemm_kernel(const __grid_constant__ GemmMaps tm, const GemmParams p) {
+  using C = TileCfg<BN>;
+  constexpr int STAGES = C::STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sA = smem;
   uint8_t* sB = smem + STAGES * A_BYTES;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
+  uint8_t* sStage = smem + STAGES * C::STAGE_BYTES;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(sStage + STAGING_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
 
   const int wg = int(threadIdx.x) >> 7;
   if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB0);
-    if (EPI == 1 || p.b_seg) { tma_prefetch_desc(&tmB1); }
-    if (p.b_seg) tma_prefetch_desc(&tmB2);
+    tma_prefetch_desc(&tm.a);
+    tma_prefetch_desc(&tm.b[0]);
+    if (EPI == 1 || p.b_seg) { tma_prefetch_desc(&tm.b[1]); }
+    if (p.b_seg) tma_prefetch_desc(&tm.b[2]);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], 8);   // one arrive per consumer warp
@@ -110,6 +118,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
 
   if (wg == 0) {
     // ===================== TMA producer =====================
+    setmaxnreg_dec<40>();
     if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
@@ -118,38 +127,39 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         decode_tile(tile, p.num_m, p.num_n, p.group, m_blk, n_blk);
         const int m0 = m_blk * BM;
         int n0 = n_blk * TN;
-        const CUtensorMap* bmap = &tmB0;
+        const CUtensorMap* bmap = &tm.b[0];
         if (p.b_seg == 1) {   // weight segment that owns these output columns
           const int sg = (n0 >= p.off1) + (n0 >= p.off2);
-          bmap = sg == 0 ? &tmB0 : (sg == 1 ? &tmB1 : &tmB2);
+          bmap = &tm.b[sg];
           n0 -= sg == 0 ? 0 : (sg == 1 ? p.off1 : p.off2);
         }
         for (int kb = 0; kb < p.num_k; ++kb) {
           mbar_wait_nocall(&empty_bar[stage], phase ^ 1);
-          mbar_arrive_expect_tx(&full_bar[stage], STAGE_BYTES);
+          mbar_arrive_expect_tx(&full_bar[stage], C::STAGE_BYTES);
           uint8_t* a_dst = sA + stage * A_BYTES;
-          uint8_t* b_dst = sB + stage * B_BYTES;
+          uint8_t* b_dst = sB + stage * C::B_BYTES;
           const int k0 = kb * BK;
           int kb0 = k0;   // k coordinate inside the selected B segment
           if (p.b_seg == 2) {
             const int sg = (k0 >= p.off1) + (k0 >= p.off2);
-            bmap = sg == 0 ? &tmB0 : (sg == 1 ? &tmB1 : &tmB2);
+            bmap = &tm.b[sg];
             kb0 = k0 - (sg == 0 ? 0 : (sg == 1 ? p.off1 : p.off2));
           }
           if (!A_MN) {
-            tma_load_2d(a_dst, &tmA, &full_bar[stage], k0, m0, p.hint_a);   // box {64 k, 128 m}
+            tma_load_2d(a_dst, &tm.a, &full_bar[stage], k0, m0, p.hint_a);   // box {64 k, 128 m}
           } else {
-            tma_load_2d(a_dst, &tmA, &full_bar[stage], m0, k0, p.hint_a);   // boxes {64 m, 64 k}
-            tma_load_2d(a_dst + 8192, &tmA, &full_bar[stage], m0 + 64, k0, p.hint_a);
+            tma_load_2d(a_dst, &tm.a, &full_bar[stage], m0, k0, p.hint_a);   // boxes {64 m, 64 k}
+            tma_load_2d(a_dst + 8192, &tm.a, &full_bar[stage], m0 + 64, k0, p.hint_a);
           }
           if (EPI == 1) {
-            tma_load_2d(b_dst, &tmB0, &full_bar[stage], k0, n0, p.hint_b);          // 64 gate rows
-            tma_load_2d(b_dst + 8192, &tmB1, &full_bar[stage], k0, n0, p.hint_b);   // 64 up rows
+            tma_load_2d(b_dst, &tm.b[0], &full_bar[stage], k0, n0, p.hint_b);                 // BN/2 gate rows
+            tma_load_2d(b_dst + C::B_BYTES / 2, &tm.b[1], &full_bar[stage], k0, n0, p.hint_b);  // BN/2 up rows
           } else if (!B_MN) {
-            tma_load_2d(b_dst, bmap, &full_bar[stage], kb0, n0, p.hint_b);          // box {64 k, 128 n}
+            tma_load_2d(b_dst, bmap, &full_bar[stage], kb0, n0, p.hint_b);                    // box {64 k, BN n}
           } else {
-            tma_load_2d(b_dst, bmap, &full_bar[stage], n0, kb0, p.hint_b);          // boxes {64 n, 64 k}
-            tma_load_2d(b_dst + 8192, bmap, &full_bar[stage], n0 + 64, kb0, p.hint_b);
+#pragma unroll
+            for (int i = 0; i < BN / 64; ++i)                                                   // boxes {64 n, 64 k}
+              tma_load_2d(b_dst + i * 8192, bmap, &full_bar[stage], n0 + 64 * i, kb0, p.hint_b);
           }
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
@@ -159,28 +169,89 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   }
 
   // ===================== consumers =====================
+  setmaxnreg_inc<232>();
   const int c = wg - 1;                          // 64-row half of the tile
   const int t = int(threadIdx.x) & 127;
   const int lane = t & 31, warp = t >> 5;
+  const int r_loc = warp * 16 + (lane >> 2);     // accumulator row inside the warpgroup's 64 (h = 0; h = 1 adds 8)
+  const int cq = 2 * (lane & 3);
+  uint8_t* stg = sStage + c * (2 * SUB_BYTES);
+  int sbuf = 0;
   int stage = 0;
   uint32_t phase = 0;
+  float acc[BN / 2];
+
+  // Staging sub-tiles out.  `fill` writes the accumulator values of one sub-tile (two for a pair) into the staging
+  // buffers; an optional `pass` then walks the staged rows coalesced (thread t: chunk t % 8 of rows t / 8 + 16 i) and
+  // combines them with global operands (residual, G / U, cos / sin), so those loads never sit next to the live
+  // accumulator.  The buffers then go to the async proxy and out as TMA stores, one bulk group per buffer.  Before a
+  // buffer is rewritten, thread 0 (bulk groups are per thread) waits until the store that last read it is done.
+  auto emit = [&](bool pair, auto&& fill, bool has_pass, auto&& pass, auto&& store) {
+    uint8_t* buf = pair ? stg : stg + sbuf * SUB_BYTES;
+    if (t == 0) {
+      if (pair) tma_store_wait_read<0>();
+      else tma_store_wait_read<1>();
+    }
+    named_bar_sync(1 + c, 128);
+    fill(buf);
+    if (has_pass) {
+      named_bar_sync(1 + c, 128);
+      pass(buf);
+    }
+    fence_proxy_async_smem();
+    named_bar_sync(1 + c, 128);
+    if (t == 0) store(buf);
+    sbuf = pair ? 0 : sbuf ^ 1;
+  };
+  auto no_pass = [](uint8_t*) {};
+  auto store1 = [&](const CUtensorMap* map, int x0, int y0) {
+    return [=](uint8_t* buf) { tma_store_2d(map, buf, x0, y0); tma_store_commit(); };
+  };
+  auto store2 = [&](const CUtensorMap* m0, int x0, const CUtensorMap* m1, int x1, int y0) {
+    return [=](uint8_t* buf) {
+      tma_store_2d(m0, buf, x0, y0); tma_store_commit();
+      tma_store_2d(m1, buf + SUB_BYTES, x1, y0); tma_store_commit();
+    };
+  };
+  // 128B swizzle of the staging rows (the TMA store map's layout): 16-byte chunk q of row r sits at chunk q ^ (r & 7);
+  // r & 7 == lane / 4 for both accumulator rows of a thread, so each warp-wide store touches all 32 banks once
+  auto put_bf16x2 = [&](uint8_t* buf, int jj, int h, uint32_t v) {   // columns 8jj + cq, +1 of a 64-column sub-tile
+    *reinterpret_cast<uint32_t*>(buf + (r_loc + 8 * h) * 128 + ((jj ^ (lane >> 2)) << 4) + 2 * cq) = v;
+  };
+  auto put_f32x2 = [&](uint8_t* buf, int jj, int h, float lo, float hi) {   // columns 8jj + cq, +1 of a 32-column one
+    const int q = 2 * jj + (cq >> 2);
+    *reinterpret_cast<float2*>(buf + (r_loc + 8 * h) * 128 + ((q ^ (lane >> 2)) << 4) + 4 * (cq & 3)) =
+        make_float2(lo, hi);
+  };
+  auto chunk = [&](uint8_t* buf, int rr) {   // the pass's 16-byte chunk (t % 8) of staged row rr
+    return reinterpret_cast<uint4*>(buf + rr * 128 + (((t & 7) ^ (rr & 7)) << 4));
+  };
+  auto stage_bf16 = [&](int s) {   // bf16-rounded accumulator columns [64s, 64s + 64)
+    return [&, s](uint8_t* buf) {
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          put_bf16x2(buf, jj, h, pack_bf16x2(acc[4 * (8 * s + jj) + 2 * h], acc[4 * (8 * s + jj) + 2 * h + 1]));
+    };
+  };
   for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
     int m_blk, n_blk;
     decode_tile(tile, p.num_m, p.num_n, p.group, m_blk, n_blk);
-    float acc[64];
 #pragma unroll
-    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
     int prev = -1;
     for (int kb = 0; kb < p.num_k; ++kb) {
       mbar_wait_nocall(&full_bar[stage], phase);
       const uint32_t a_addr = smem_u32(sA + stage * A_BYTES) + uint32_t(c) * 8192u;
-      const uint32_t b_addr = smem_u32(sB + stage * B_BYTES);
+      const uint32_t b_addr = smem_u32(sB + stage * C::B_BYTES);
       wgmma_fence();
 #pragma unroll
       for (int k = 0; k < BK / 16; ++k) {
         const uint64_t da = A_MN ? make_sdesc_sw128(a_addr + k * 2048, 8192, 1024) : make_sdesc_sw128(a_addr + k * 32, 16, 1024);
         const uint64_t db = B_MN ? make_sdesc_sw128(b_addr + k * 2048, 8192, 1024) : make_sdesc_sw128(b_addr + k * 32, 16, 1024);
-        wgmma_m64n128<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, 1u);
+        if constexpr (BN == 256) wgmma_m64n256<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, 1u);
+        else wgmma_m64n128<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, 1u);
       }
       wgmma_commit();
       wgmma_wait<1>();                           // the previous k-block's MMAs have retired: its slot can be refilled
@@ -193,141 +264,230 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     wgmma_fence_regs(acc);
     if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
 
-    // ---------------- epilogue: registers -> global ----------------
+    // ---------------- epilogue: registers -> swizzled staging (-> coalesced pass) -> TMA store ----------------
     const int m0 = m_blk * BM;
     const int n0 = n_blk * TN;
-    const int row_base = m0 + c * 64 + warp * 16 + (lane >> 2);
-    const int cq = 2 * (lane & 3);
+    const int y0 = m0 + c * 64;                  // first row of this warpgroup; the stores clip rows >= M, cols >= N
+    if (y0 >= p.M) continue;                     // warpgroup-uniform
     if (EPI == 1) {
-      bf16* H = static_cast<bf16*>(p.D[0]);
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
+      for (int s = 0; s < TN / 64; ++s) {
+        const int x0 = n0 + 64 * s;
+        if (x0 >= p.N) break;
+        // mimic the unfused reference rounding: g,u -> bf16; silu(g) -> bf16; * u -> bf16
+        auto gate = [&](int jj, int h, int e) { return bf16_round(acc[4 * (8 * s + jj) + 2 * h + e]); };
+        auto up = [&](int jj, int h, int e) { return bf16_round(acc[4 * (8 * s + jj + BN / 16) + 2 * h + e]); };
+        emit(false, [&](uint8_t* buf) {
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int row = row_base + 8 * h, col = n0 + 8 * j + cq;
-          if (row >= p.M || col >= p.N) continue;
-          // mimic the unfused reference rounding: g,u -> bf16; silu(g) -> bf16; * u -> bf16
-          float g[2], u[2], hh[2];
+          for (int jj = 0; jj < 8; ++jj)
 #pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            g[e] = bf16_round(acc[4 * j + 2 * h + e]);
-            u[e] = bf16_round(acc[4 * (j + 8) + 2 * h + e]);
-            hh[e] = bf16_round(g[e] / (1.f + __expf(-g[e]))) * u[e];
-          }
-          const int64_t off = int64_t(row) * p.ldd + col;
-          st_bf16x2(H + off, col, p.N, hh[0], hh[1]);
-          if (p.G) st_bf16x2(p.G + off, col, p.N, g[0], g[1]);
-          if (p.U) st_bf16x2(p.U + off, col, p.N, u[0], u[1]);
-        }
+            for (int h = 0; h < 2; ++h) {
+              float hh[2];
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const float g = gate(jj, h, e);
+                hh[e] = bf16_round(g / (1.f + __expf(-g))) * up(jj, h, e);
+              }
+              put_bf16x2(buf, jj, h, pack_bf16x2(hh[0], hh[1]));
+            }
+        }, false, no_pass, store1(&tm.d[0], x0, y0));
+        if (p.has_g)
+          emit(false, [&](uint8_t* buf) {
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+              for (int h = 0; h < 2; ++h) put_bf16x2(buf, jj, h, pack_bf16x2(gate(jj, h, 0), gate(jj, h, 1)));
+          }, false, no_pass, store1(&tm.d[1], x0, y0));
+        if (p.has_u)
+          emit(false, [&](uint8_t* buf) {
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+              for (int h = 0; h < 2; ++h) put_bf16x2(buf, jj, h, pack_bf16x2(up(jj, h, 0), up(jj, h, 1)));
+          }, false, no_pass, store1(&tm.d[2], x0, y0));
       }
     } else if (EPI == 3) {
-      bf16* dG = static_cast<bf16*>(p.D[0]);
-      bf16* dU = static_cast<bf16*>(p.D[1]);
+      // dH (bf16-rounded, as the unfused path stores it) staged in buffer 0; the pass reads it with G / U and writes dG
+      // over it and dU into buffer 1
 #pragma unroll
-      for (int j = 0; j < 16; ++j) {
+      for (int s = 0; s < BN / 64; ++s) {
+        const int x0 = n0 + 64 * s;
+        if (x0 >= p.N) break;
+        emit(true, stage_bf16(s), true, [&](uint8_t* buf) {
+          // 4-byte pieces (a warp per row): next to the live accumulator there is no room for wider ones
+#pragma unroll 1
+          for (int i = 0; i < 16; ++i) {
+            const int rr = (t >> 5) + 4 * i, row = y0 + rr, col = x0 + 2 * lane;
+            if (row >= p.M || col >= p.N) continue;   // N % 8 == 0: whole pairs
+            const int off = rr * 128 + (((lane >> 2) ^ (rr & 7)) << 4) + 4 * (lane & 3);
+            uint32_t* pd = reinterpret_cast<uint32_t*>(buf + off);
+            uint32_t* pu = reinterpret_cast<uint32_t*>(buf + SUB_BYTES + off);
+            const uint32_t dw = *pd;
+            const uint32_t gw = *reinterpret_cast<const uint32_t*>(p.aux_g + int64_t(row) * p.ld_gu + col);
+            const uint32_t uw = *reinterpret_cast<const uint32_t*>(p.aux_u + int64_t(row) * p.ld_gu + col);
+            float rg[2], ru[2];
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int row = row_base + 8 * h, col = n0 + 8 * j + cq;
-          if (row >= p.M || col >= p.N) continue;   // N % 8 == 0: col < N -> col + 1 < N
-          const uint32_t gw = *reinterpret_cast<const uint32_t*>(p.aux_g + int64_t(row) * p.ld_gu + col);
-          const uint32_t uw = *reinterpret_cast<const uint32_t*>(p.aux_u + int64_t(row) * p.ld_gu + col);
-          float rg[2], ru[2];
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const float g = e ? bf16hi(gw) : bf16lo(gw);
-            const float u = e ? bf16hi(uw) : bf16lo(uw);
-            const float dh = bf16_round(acc[4 * j + 2 * h + e]);   // the bf16 dH the unfused path stores
-            const float sig = 1.f / (1.f + __expf(-g));
-            const float silu = g * sig;
-            ru[e] = dh * bf16_round(silu);
-            rg[e] = bf16_round(dh * u) * (sig * (1.f + g * (1.f - sig)));
+            for (int e = 0; e < 2; ++e) {
+              const float d = e ? bf16hi(dw) : bf16lo(dw);
+              const float g = e ? bf16hi(gw) : bf16lo(gw);
+              const float u = e ? bf16hi(uw) : bf16lo(uw);
+              const float sig = 1.f / (1.f + __expf(-g));
+              ru[e] = d * bf16_round(g * sig);
+              rg[e] = bf16_round(d * u) * (sig * (1.f + g * (1.f - sig)));
+            }
+            *pd = pack_bf16x2(rg[0], rg[1]);
+            *pu = pack_bf16x2(ru[0], ru[1]);
           }
-          const int64_t off = int64_t(row) * p.ldd + col;
-          *reinterpret_cast<uint32_t*>(dG + off) = pack_bf16x2(rg[0], rg[1]);
-          *reinterpret_cast<uint32_t*>(dU + off) = pack_bf16x2(ru[0], ru[1]);
-        }
+        }, store2(&tm.d[0], x0, &tm.d[1], x0, y0));
       }
     } else if (EPI == 0 && p.rope_cos != nullptr && n0 < p.rope_end) {
-      // RoPE tile: one head of 128 columns; pairs (j, j+64) sit in accumulator groups j and j+8 of this thread
-      bf16* D = static_cast<bf16*>(p.D[0]);
+      // RoPE tile: BN / 128 whole heads.  Both halves of a head (columns j and j + 64 pair up) are staged as bf16, then
+      // the pass rotates them with the row's cos / sin and writes o1 over the first half and o2 over the second.
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
+      for (int hd = 0; hd < BN / 128; ++hd) {
+        const int x0 = n0 + 128 * hd;
+        emit(true, [&](uint8_t* buf) {
+          stage_bf16(2 * hd)(buf);
+          stage_bf16(2 * hd + 1)(buf + SUB_BYTES);
+        }, true, [&](uint8_t* buf) {
+#pragma unroll 1
+          for (int i = 0; i < 4; ++i) {
+            const int rr = (t >> 3) + 16 * i, row = y0 + rr, cc = 8 * (t & 7);
+            if (row >= p.M) continue;
+            uint4* pa = chunk(buf, rr);
+            uint4* pb = chunk(buf + SUB_BYTES, rr);
+            const uint4 av = *pa, bv = *pb;
+            const uint4 cv = *reinterpret_cast<const uint4*>(p.rope_cos + int64_t(row) * 64 + cc);
+            const uint4 sv = *reinterpret_cast<const uint4*>(p.rope_sin + int64_t(row) * 64 + cc);
+            const uint32_t* aw = &av.x;
+            const uint32_t* bw = &bv.x;
+            const uint32_t* cw = &cv.x;
+            const uint32_t* sw = &sv.x;
+            uint4 o1, o2;
+            uint32_t* o1w = &o1.x;
+            uint32_t* o2w = &o2.x;
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int row = row_base + 8 * h, cc = 8 * j + cq;
-          if (row >= p.M) continue;
-          const uint32_t cw = *reinterpret_cast<const uint32_t*>(p.rope_cos + int64_t(row) * 64 + cc);
-          const uint32_t sw = *reinterpret_cast<const uint32_t*>(p.rope_sin + int64_t(row) * 64 + cc);
-          float o1[2], o2[2];
+            for (int w = 0; w < 4; ++w) {
+              float r1[2], r2[2];
 #pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const float a = bf16_round(acc[4 * j + 2 * h + e]), b = bf16_round(acc[4 * (j + 8) + 2 * h + e]);
-            const float cs = e ? bf16hi(cw) : bf16lo(cw), sn = e ? bf16hi(sw) : bf16lo(sw);
-            o1[e] = bf16_round(a * cs) + bf16_round(-b * sn);
-            o2[e] = bf16_round(b * cs) + bf16_round(a * sn);
+              for (int e = 0; e < 2; ++e) {
+                const float a = e ? bf16hi(aw[w]) : bf16lo(aw[w]), b = e ? bf16hi(bw[w]) : bf16lo(bw[w]);
+                const float cs = e ? bf16hi(cw[w]) : bf16lo(cw[w]), sn = e ? bf16hi(sw[w]) : bf16lo(sw[w]);
+                r1[e] = bf16_round(a * cs) + bf16_round(-b * sn);
+                r2[e] = bf16_round(b * cs) + bf16_round(a * sn);
+              }
+              o1w[w] = pack_bf16x2(r1[0], r1[1]);
+              o2w[w] = pack_bf16x2(r2[0], r2[1]);
+            }
+            *pa = o1;
+            *pb = o2;
           }
-          const int64_t off = int64_t(row) * p.ldd + n0 + cc;
-          *reinterpret_cast<uint32_t*>(D + off) = pack_bf16x2(o1[0], o1[1]);
-          *reinterpret_cast<uint32_t*>(D + off + 64) = pack_bf16x2(o2[0], o2[1]);
-        }
+        }, store2(&tm.d[0], x0, &tm.d[0], x0 + 64, y0));
       }
     } else {
-      void* Dbase = p.D[0];
-      int drow_off = 0;
+      const CUtensorMap* dmap = &tm.d[0];
+      int yd = y0;
       if (p.d_seg == 1) {   // output rows belong to one of several gradient tensors (segments are multiples of 256)
         const int sg = (m0 >= p.off1) + (m0 >= p.off2);
-        Dbase = p.D[sg];
-        drow_off = sg == 0 ? 0 : (sg == 1 ? p.off1 : p.off2);
+        dmap = &tm.d[sg];
+        yd -= sg == 0 ? 0 : (sg == 1 ? p.off1 : p.off2);
       }
+      constexpr int SW = EPI == 2 ? 32 : 64;   // columns per sub-tile
+      constexpr int CW = SW / 8;               // columns per 16-byte chunk
 #pragma unroll
-      for (int j = 0; j < 16; ++j) {
+      for (int s = 0; s < BN / SW; ++s) {
+        const int x0 = n0 + SW * s;
+        if (x0 >= p.N) break;
+        auto fill = [&](uint8_t* buf) {
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int row = row_base + 8 * h, col = n0 + 8 * j + cq;
-          if (row >= p.M || col >= p.N) continue;
-          float lo = acc[4 * j + 2 * h], hi = acc[4 * j + 2 * h + 1];
-          const int64_t doff = int64_t(row - drow_off) * p.ldd + col;
-          const int64_t roff = int64_t(row) * p.ldr + col;
-          const bool two = col + 1 < p.N;
-          if (EPI == 2) {
-            float* dp = static_cast<float*>(Dbase) + doff;
-            if (p.R) {
-              const float* rp = static_cast<const float*>(p.R) + roff;
-              lo += rp[0];
-              if (two) hi += rp[1];
+          for (int jj = 0; jj < SW / 8; ++jj)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const float lo = acc[4 * ((SW / 8) * s + jj) + 2 * h], hi = acc[4 * ((SW / 8) * s + jj) + 2 * h + 1];
+              if (EPI == 2) put_f32x2(buf, jj, h, lo, hi);
+              else put_bf16x2(buf, jj, h, pack_bf16x2(lo, hi));
             }
-            if (two) *reinterpret_cast<float2*>(dp) = make_float2(lo, hi);
-            else dp[0] = lo;
-          } else {
-            bf16* dp = static_cast<bf16*>(Dbase) + doff;
-            if (p.R) {
-              // reference order: matmul result rounded to bf16, then bf16 add with the residual
-              const bf16* rp = static_cast<const bf16*>(p.R) + roff;
-              lo = bf16_round(lo) + __bfloat162float(rp[0]);
-              if (two) hi = bf16_round(hi) + __bfloat162float(rp[1]);
+        };
+        // + R: fp32 acc + R, or (reference order) the bf16-rounded product + R rounded again
+        auto add_residual = [&](uint8_t* buf) {
+#pragma unroll 1
+          for (int i = 0; i < 4; ++i) {
+            const int rr = (t >> 3) + 16 * i, row = y0 + rr, col = x0 + CW * (t & 7);
+            if (row >= p.M || col >= p.N) continue;
+            uint4* pd = chunk(buf, rr);
+            uint4 v = *pd;
+            if (EPI == 2) {
+              const float* rp = static_cast<const float*>(p.R) + int64_t(row) * p.ldr + col;
+              float* f = reinterpret_cast<float*>(&v);
+              if (col + 4 <= p.N) {
+                const float4 r = *reinterpret_cast<const float4*>(rp);
+                f[0] += r.x; f[1] += r.y; f[2] += r.z; f[3] += r.w;
+              } else {
+#pragma unroll
+                for (int e = 0; e < 4; ++e)
+                  if (col + e < p.N) f[e] += rp[e];
+              }
+            } else {
+              const bf16* rp = static_cast<const bf16*>(p.R) + int64_t(row) * p.ldr + col;
+              uint4 r = make_uint4(0, 0, 0, 0);
+              uint32_t* rw = &r.x;
+              if (col + 8 <= p.N) {
+                r = *reinterpret_cast<const uint4*>(rp);
+              } else {   // ragged N: the pairs that exist (the columns past N are clipped by the store)
+#pragma unroll
+                for (int e = 0; e < 8; e += 2)
+                  if (col + e < p.N)
+                    rw[e / 2] = uint32_t(__bfloat16_as_ushort(rp[e])) |
+                                (col + e + 1 < p.N ? uint32_t(__bfloat16_as_ushort(rp[e + 1])) << 16 : 0u);
+              }
+              uint32_t* vw = &v.x;
+#pragma unroll
+              for (int w = 0; w < 4; ++w)
+                vw[w] = pack_bf16x2(bf16lo(vw[w]) + bf16lo(rw[w]), bf16hi(vw[w]) + bf16hi(rw[w]));
             }
-            st_bf16x2(dp, col, p.N, lo, hi);
+            *pd = v;
           }
-        }
+        };
+        emit(false, fill, p.R != nullptr, add_residual, store1(dmap, x0, yd));
       }
     }
   }
+  if (t == 0) tma_store_wait<0>();   // staging must stay valid until the last stores have read it
 }
 
-template <bool A_MN, bool B_MN, int EPI>
-static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB0, const CUtensorMap& tmB1, const CUtensorMap& tmB2,
-                       const GemmParams& p, cudaStream_t stream) {
-  auto kern = gemm_kernel<A_MN, B_MN, EPI>;
+template <int BN, bool A_MN, bool B_MN, int EPI>
+static int launch_gemm(const GemmMaps& tm, const GemmParams& p, cudaStream_t stream) {
+  auto kern = gemm_kernel<BN, A_MN, B_MN, EPI>;
+  constexpr int smem = TileCfg<BN>::SMEM;
   static bool configured = false;  // per instantiation
   if (!configured) {
-    TN_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM));
+    TN_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     configured = true;
   }
   const int tiles = p.num_m * p.num_n;
   const int grid = tiles < sm_count() ? tiles : sm_count();
-  kern<<<grid, GEMM_THREADS, GEMM_SMEM, stream>>>(tmA, tmB0, tmB1, tmB2, p);
+  kern<<<grid, GEMM_THREADS, smem, stream>>>(tm, p);
   TN_CHECK_CUDA(cudaGetLastError());
   return TN_OK;
+}
+
+template <bool A_MN, bool B_MN, int EPI>
+static int launch_gemm(int bn, const GemmMaps& tm, const GemmParams& p, cudaStream_t stream) {
+  return bn == 256 ? launch_gemm<256, A_MN, B_MN, EPI>(tm, p, stream) : launch_gemm<128, A_MN, B_MN, EPI>(tm, p, stream);
+}
+
+// Tile width from the shape: a 128x256 tile does the work of two 128x128 tiles in kWideTileCost of the time of one, so
+// the wide tile wins unless halving the tile count costs more in the last, partly idle wave than it saves per tile
+// (e.g. 3072x3072: 576 narrow tiles in 5 waves vs 288 wide tiles in 3).  `out_div` = accumulator columns per output
+// column (2 for SwiGLU).  A pure function of the shape, so equal shapes always get equal tiles.
+constexpr double kWideTileCost = 1.8;
+static int pick_bn(int M, int N, int out_div) {
+  const int64_t sms = sm_count();
+  const int64_t nm = (M + BM - 1) / BM;
+  const int64_t wide = nm * ((N + 256 / out_div - 1) / (256 / out_div));
+  const int64_t narrow = nm * ((N + 128 / out_div - 1) / (128 / out_div));
+  const int64_t w_wide = (wide + sms - 1) / sms, w_narrow = (narrow + sms - 1) / sms;
+  return double(w_wide) * kWideTileCost <= double(w_narrow) ? 256 : 128;
 }
 
 static GemmParams base_params(int M, int N, int K, int tile_n) {
@@ -350,6 +510,11 @@ static int map_operand(CUtensorMap* m, const void* ptr, int mn, uint64_t rows, u
   return encode_tmap_2d(m, ptr, 2, rows, K, uint64_t(ld) * 2, 64, 64, true);
 }
 
+// output [rows, cols] (row stride ld elements) -> box of one staging sub-tile: 64 rows x (64 bf16 | 32 fp32) columns
+static int map_output(CUtensorMap* m, const void* ptr, int f32, uint64_t rows, uint64_t cols, int64_t ld) {
+  return encode_tmap_2d(m, ptr, f32 ? 4 : 2, cols, rows, uint64_t(ld) * (f32 ? 4 : 2), f32 ? 32 : 64, 64, true);
+}
+
 }  // namespace tn
 
 using namespace tn;
@@ -367,16 +532,20 @@ extern "C" int tn_gemm_bf16(const void* A, int64_t lda, int a_mn, const void* B,
              "tn_gemm_bf16: D/R must be 16 B aligned");
   TN_REQUIRE(!(a_mn && !b_mn), "tn_gemm_bf16: (a_mn=1, b_mn=0) layout is not instantiated");
 
-  GemmParams p = base_params(M, N, K, BN);
-  p.D[0] = D; p.ldd = ldd; p.R = R; p.ldr = ldr;
-  CUtensorMap tmA, tmB;
+  const int bn = pick_bn(M, N, 1);
+  GemmParams p = base_params(M, N, K, bn);
+  p.R = R; p.ldr = ldr;
+  GemmMaps tm;
   int rc;
-  if ((rc = map_operand(&tmA, A, a_mn, uint64_t(M), uint64_t(K), lda, BM))) return rc;
-  if ((rc = map_operand(&tmB, B, b_mn, uint64_t(N), uint64_t(K), ldb, BN))) return rc;
+  if ((rc = map_operand(&tm.a, A, a_mn, uint64_t(M), uint64_t(K), lda, BM))) return rc;
+  if ((rc = map_operand(&tm.b[0], B, b_mn, uint64_t(N), uint64_t(K), ldb, bn))) return rc;
+  if ((rc = map_output(&tm.d[0], D, d_f32, uint64_t(M), uint64_t(N), ldd))) return rc;
+  tm.b[1] = tm.b[2] = tm.b[0];
+  tm.d[1] = tm.d[2] = tm.d[0];
 
-#define TN_GEMM_DISPATCH(AMN_, BMN_)                                        \
-  (d_f32 ? launch_gemm<AMN_, BMN_, 2>(tmA, tmB, tmB, tmB, p, stream)        \
-         : launch_gemm<AMN_, BMN_, 0>(tmA, tmB, tmB, tmB, p, stream))
+#define TN_GEMM_DISPATCH(AMN_, BMN_)                              \
+  (d_f32 ? launch_gemm<AMN_, BMN_, 2>(bn, tm, p, stream)          \
+         : launch_gemm<AMN_, BMN_, 0>(bn, tm, p, stream))
   if (!a_mn && !b_mn) return TN_GEMM_DISPATCH(false, false);
   if (!a_mn && b_mn) return TN_GEMM_DISPATCH(false, true);
   return TN_GEMM_DISPATCH(true, true);
@@ -393,15 +562,20 @@ extern "C" int tn_gemm_swiglu_bf16(const void* X, int64_t ldx, const void* Wg, c
   TN_REQUIRE((reinterpret_cast<uintptr_t>(H) & 15) == 0 && (!G || (reinterpret_cast<uintptr_t>(G) & 15) == 0) &&
                  (!U || (reinterpret_cast<uintptr_t>(U) & 15) == 0),
              "tn_gemm_swiglu_bf16: outputs must be 16 B aligned");
-  GemmParams p = base_params(M, N, K, BN / 2);
-  p.D[0] = H; p.ldd = ldh;
-  p.G = static_cast<bf16*>(G); p.U = static_cast<bf16*>(U);
-  CUtensorMap tmA, tmG, tmU;
+  const int bn = pick_bn(M, N, 2);
+  GemmParams p = base_params(M, N, K, bn / 2);
+  p.has_g = G != nullptr; p.has_u = U != nullptr;
+  GemmMaps tm;
   int rc;
-  if ((rc = map_operand(&tmA, X, 0, uint64_t(M), uint64_t(K), ldx, BM))) return rc;
-  if ((rc = map_operand(&tmG, Wg, 0, uint64_t(N), uint64_t(K), ldw, BN / 2))) return rc;
-  if ((rc = map_operand(&tmU, Wu, 0, uint64_t(N), uint64_t(K), ldw, BN / 2))) return rc;
-  return launch_gemm<false, false, 1>(tmA, tmG, tmU, tmU, p, stream);
+  if ((rc = map_operand(&tm.a, X, 0, uint64_t(M), uint64_t(K), ldx, BM))) return rc;
+  if ((rc = map_operand(&tm.b[0], Wg, 0, uint64_t(N), uint64_t(K), ldw, bn / 2))) return rc;
+  if ((rc = map_operand(&tm.b[1], Wu, 0, uint64_t(N), uint64_t(K), ldw, bn / 2))) return rc;
+  tm.b[2] = tm.b[1];
+  if ((rc = map_output(&tm.d[0], H, 0, uint64_t(M), uint64_t(N), ldh))) return rc;
+  tm.d[1] = tm.d[2] = tm.d[0];
+  if (G && (rc = map_output(&tm.d[1], G, 0, uint64_t(M), uint64_t(N), ldh))) return rc;
+  if (U && (rc = map_output(&tm.d[2], U, 0, uint64_t(M), uint64_t(N), ldh))) return rc;
+  return launch_gemm<false, false, 1>(bn, tm, p, stream);
 }
 
 // Down-proj dgrad with the SwiGLU backward in its epilogue: dH = dY[M,K].W[K,N] (W = down_proj.weight [d, ffn], MN-major B),
@@ -417,14 +591,18 @@ extern "C" int tn_gemm_dswiglu_bf16(const void* dY, int64_t lddy, const void* W,
              "tn_gemm_dswiglu_bf16: leading dims and N must be multiples of 8");
   TN_REQUIRE(((reinterpret_cast<uintptr_t>(G) | reinterpret_cast<uintptr_t>(U) | reinterpret_cast<uintptr_t>(dG) |
                reinterpret_cast<uintptr_t>(dU)) & 15) == 0, "tn_gemm_dswiglu_bf16: G, U, dG, dU must be 16 B aligned");
-  GemmParams p = base_params(M, N, K, BN);
-  p.D[0] = dG; p.D[1] = dU; p.ldd = lddg;
+  const int bn = pick_bn(M, N, 1);   // the tile tn_gemm_bf16 would use for dH
+  GemmParams p = base_params(M, N, K, bn);
   p.aux_g = static_cast<const bf16*>(G); p.aux_u = static_cast<const bf16*>(U); p.ld_gu = ldgu;
-  CUtensorMap tmA, tmB;
+  GemmMaps tm;
   int rc;
-  if ((rc = map_operand(&tmA, dY, 0, uint64_t(M), uint64_t(K), lddy, BM))) return rc;
-  if ((rc = map_operand(&tmB, W, 1, uint64_t(N), uint64_t(K), ldw, BN))) return rc;
-  return launch_gemm<false, true, 3>(tmA, tmB, tmB, tmB, p, stream);
+  if ((rc = map_operand(&tm.a, dY, 0, uint64_t(M), uint64_t(K), lddy, BM))) return rc;
+  if ((rc = map_operand(&tm.b[0], W, 1, uint64_t(N), uint64_t(K), ldw, bn))) return rc;
+  tm.b[1] = tm.b[2] = tm.b[0];
+  if ((rc = map_output(&tm.d[0], dG, 0, uint64_t(M), uint64_t(N), lddg))) return rc;
+  if ((rc = map_output(&tm.d[1], dU, 0, uint64_t(M), uint64_t(N), lddg))) return rc;
+  tm.d[2] = tm.d[1];
+  return launch_gemm<false, true, 3>(bn, tm, p, stream);
 }
 
 // Three weights / gradients treated as one operand (see GemmParams).  mode: 0 = forward  D[M, n0+n1+n2] = A·[B0;B1;B2]ᵀ
@@ -450,10 +628,10 @@ extern "C" int tn_gemm_qkv_bf16(int mode, const void* A, int64_t lda, const void
   TN_REQUIRE(rope_cos == nullptr || mode == 0, "tn_gemm_qkv_bf16: fused RoPE exists for the forward projection only");
   const void* Bs[3] = {B0, B1, B2};
   const int seg[3] = {s0, s1, s2};
-  GemmParams p = base_params(M, N, K, BN);
+  const int bn = pick_bn(M, N, 1);
+  GemmParams p = base_params(M, N, K, bn);
   p.off1 = s0; p.off2 = s0 + s1;
-  p.D[0] = D0; p.ldd = ldd;
-  CUtensorMap tmA, tmB[3];
+  GemmMaps tm;
   int rc;
   if (mode == 0) {
     if (rope_cos) {
@@ -461,22 +639,28 @@ extern "C" int tn_gemm_qkv_bf16(int mode, const void* A, int64_t lda, const void
       p.rope_end = s0 + s1;
     }
     p.b_seg = 1;
-    if ((rc = map_operand(&tmA, A, 0, uint64_t(M), uint64_t(K), lda, BM))) return rc;
+    if ((rc = map_operand(&tm.a, A, 0, uint64_t(M), uint64_t(K), lda, BM))) return rc;
     for (int i = 0; i < 3; ++i)
-      if ((rc = map_operand(&tmB[i], Bs[i], 0, uint64_t(seg[i]), uint64_t(K), ldb, BN))) return rc;
-    return launch_gemm<false, false, 0>(tmA, tmB[0], tmB[1], tmB[2], p, stream);
+      if ((rc = map_operand(&tm.b[i], Bs[i], 0, uint64_t(seg[i]), uint64_t(K), ldb, bn))) return rc;
+    if ((rc = map_output(&tm.d[0], D0, 0, uint64_t(M), uint64_t(N), ldd))) return rc;
+    tm.d[1] = tm.d[2] = tm.d[0];
+    return launch_gemm<false, false, 0>(bn, tm, p, stream);
   }
   if (mode == 1) {
     p.b_seg = 2;
-    if ((rc = map_operand(&tmA, A, 0, uint64_t(M), uint64_t(K), lda, BM))) return rc;
+    if ((rc = map_operand(&tm.a, A, 0, uint64_t(M), uint64_t(K), lda, BM))) return rc;
     for (int i = 0; i < 3; ++i)   // B_i stored [seg_i (K), N] row-major, N contiguous
-      if ((rc = map_operand(&tmB[i], Bs[i], 1, uint64_t(N), uint64_t(seg[i]), ldb, BN))) return rc;
-    return launch_gemm<false, true, 0>(tmA, tmB[0], tmB[1], tmB[2], p, stream);
+      if ((rc = map_operand(&tm.b[i], Bs[i], 1, uint64_t(N), uint64_t(seg[i]), ldb, bn))) return rc;
+    if ((rc = map_output(&tm.d[0], D0, 0, uint64_t(M), uint64_t(N), ldd))) return rc;
+    tm.d[1] = tm.d[2] = tm.d[0];
+    return launch_gemm<false, true, 0>(bn, tm, p, stream);
   }
   p.d_seg = 1;
-  p.D[1] = D1; p.D[2] = D2;
-  if ((rc = map_operand(&tmA, A, 1, uint64_t(M), uint64_t(K), lda, BM))) return rc;
-  if ((rc = map_operand(&tmB[0], B0, 1, uint64_t(N), uint64_t(K), ldb, BN))) return rc;
-  return d_f32 ? launch_gemm<true, true, 2>(tmA, tmB[0], tmB[0], tmB[0], p, stream)
-               : launch_gemm<true, true, 0>(tmA, tmB[0], tmB[0], tmB[0], p, stream);
+  void* Ds[3] = {D0, D1, D2};
+  if ((rc = map_operand(&tm.a, A, 1, uint64_t(M), uint64_t(K), lda, BM))) return rc;
+  if ((rc = map_operand(&tm.b[0], B0, 1, uint64_t(N), uint64_t(K), ldb, bn))) return rc;
+  tm.b[1] = tm.b[2] = tm.b[0];
+  for (int i = 0; i < 3; ++i)   // one map per gradient tensor [seg_i, N]
+    if ((rc = map_output(&tm.d[i], Ds[i], d_f32, uint64_t(seg[i]), uint64_t(N), ldd))) return rc;
+  return d_f32 ? launch_gemm<true, true, 2>(bn, tm, p, stream) : launch_gemm<true, true, 0>(bn, tm, p, stream);
 }
