@@ -139,6 +139,36 @@ int tn_attn_bwd_bf16(const void* Q, int64_t ldq, const void* K, int64_t ldk, con
                      const void* rope_sin_q, const void* rope_cos_k, const void* rope_sin_k, tn_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
+ * Autoregressive decoding (touchnet_b200/generation.py).  Reference interface: the greedy `model.generate(use_cache=True,
+ * do_sample=False, num_beams=1, repetition_penalty, no_repeat_ngram_size, ...)` of
+ * touchnet/models/touch_audio/inference_touch_audio.py:170-192 (hf: DynamicCache + sdpa attention of the new token,
+ * RepetitionPenaltyLogitsProcessor, NoRepeatNGramLogitsProcessor, argmax).
+ *   Cache K/V: [B, S_cap, KV, 128] bf16 with token stride ld_tok and batch stride ld_batch (elements).
+ *   tn_attn_decode: one query row per batch row, Q [B, H*128] (row stride ldq, RoPE already applied) against cache rows
+ *     [kv_start[b], kv_end[b]) (device int32).  Split-KV: the split count depends on (B, KV, S_cap) only; `workspace`
+ *     holds tn_attn_decode_ws_floats(B, H, KV, S_cap) floats.  O [B, H*128] bf16; lse [B, H] fp32 (optional, natural
+ *     log) with the conventions of tn_attn_fwd_bf16 (O = 0, lse = +inf for an empty range).  H/KV in 1..16.
+ *     Bit-reproducible (splits are merged in a fixed order).
+ *   tn_kv_append: cache rows [row_end[b] - T_new, row_end[b]) of batch row b <- source rows b*T_new .. b*T_new+T_new-1 of
+ *     K / V (row strides ldk / ldv, `width` = KV*128 columns copied).
+ *   tn_greedy_select: per row b, over the bf16 logits [B, V] (row stride ld) cast to fp32: repetition penalty on every id
+ *     of history[b, 0:length[b]] (score < 0 ? score*p : score/p), no-repeat-ngram ban (n = no_repeat_ngram_size, 0 = off),
+ *     argmax (lowest index on ties); finished rows take `pad`.  Then history[b, length[b]] = next_ids[b] = token,
+ *     length[b] += 1, positions[b] += 1, finished[b] |= (token == eos).
+ */
+int64_t tn_attn_decode_ws_floats(int B, int H, int KV, int S_cap);
+int tn_attn_decode_bf16(const void* Q, int64_t ldq, const void* K, const void* V, int64_t ld_tok, int64_t ld_batch,
+                        const int32_t* kv_start, const int32_t* kv_end, int B, int H, int KV, int S_cap, float scale,
+                        float* workspace, void* O, int64_t ldo, float* lse, tn_stream_t stream);
+int tn_kv_append_bf16(const void* K, int64_t ldk, const void* V, int64_t ldv, void* K_cache, void* V_cache,
+                      int64_t ld_tok, int64_t ld_batch, const int32_t* row_end, int B, int T_new, int S_cap, int width,
+                      tn_stream_t stream);
+int tn_greedy_select_bf16(const void* logits, int64_t ld, int B, int V, int64_t* history, int64_t ld_hist,
+                          int32_t* length, int64_t* positions, int64_t* next_ids, int32_t* finished,
+                          float repetition_penalty, int no_repeat_ngram_size, int64_t eos, int64_t pad,
+                          tn_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------------------------
  * Audio frontend.
  *   tn_fbank: touchnet/data/functions.py:117-134 audio_compute_fbank → ta:compliance/kaldi.py:514-645 (snip_edges,
  *     remove DC, pre-emphasis, povey window, |rfft|², HTK mel bank, log) batched over utterances packed back to back.

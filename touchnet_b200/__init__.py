@@ -6,4 +6,4 @@ __version__ = "0.1.0"
 from . import _lib  # noqa: F401
 
 __all__ = ["_lib", "ops", "modeling", "frontend", "batching", "loss", "tokenizer", "optim", "train_spec", "parallelize",
-           "tensor_parallel", "context_parallel", "fsdp_comm"]
+           "tensor_parallel", "context_parallel", "fsdp_comm", "generation"]

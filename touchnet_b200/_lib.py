@@ -40,6 +40,10 @@ _SIGNATURES = {
     "tn_attn_fwd_bf16": [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _vp, _vp, _i, _i, _i, _i, _f, _i, _i, _vp],
     "tn_attn_bwd_bf16": [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _vp, _vp, _i64, _vp, _i64,
                          _vp, _i64, _vp, _vp, _i, _i, _i, _i, _f, _i, _i, _vp, _vp, _vp, _vp, _vp],
+    "tn_attn_decode_ws_floats": [_i, _i, _i, _i],
+    "tn_attn_decode_bf16": [_vp, _i64, _vp, _vp, _i64, _i64, _vp, _vp, _i, _i, _i, _i, _f, _vp, _vp, _i64, _vp, _vp],
+    "tn_kv_append_bf16": [_vp, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _vp, _i, _i, _i, _i, _vp],
+    "tn_greedy_select_bf16": [_vp, _i64, _i, _i, _vp, _i64, _vp, _vp, _vp, _vp, _f, _i, _i64, _i64, _vp],
     "tn_fbank_f32": [_vp, _i, _vp, _vp, _i, _i64, _i, _i, _i, _vp, _vp, _i, _f, _vp, _vp],
     "tn_logmel_power_f32": [_vp, _vp, _vp, _i, _i64, _i, _i, _vp, _vp, _i, _vp, _vp, _vp],
     "tn_logmel_finish_f32": [_vp, _vp, _vp, _i, _i64, _i, _vp],
@@ -61,7 +65,7 @@ _SIGNATURES = {
     "tn_pack_ce_fused_bf16": [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _f, _i64, _i, _vp],
     "tn_adamw_f32": [_vp, _vp, _vp, _vp, _vp, _i64, _f, _f, _f, _f, _f, _f, _f, _vp, _vp],
 }
-_RESTYPES = {"tn_last_error": c_char_p, "tn_attn_meta_ints": c_int64}
+_RESTYPES = {"tn_last_error": c_char_p, "tn_attn_meta_ints": c_int64, "tn_attn_decode_ws_floats": c_int64}
 
 EXPORTED_SYMBOLS = sorted(list(_SIGNATURES) + ["tn_last_error"])
 
@@ -95,8 +99,8 @@ def load(path: str | None = None) -> ctypes.CDLL:
 
 
 # kernels launched per entry point (for bench.py's `gpu_launches` claim)
-_LAUNCHES = {"tn_attn_prep": 3, "tn_attn_bwd_bf16": 3, "tn_logmel_power_f32": 2, "tn_rmsnorm_bwd_bf16": 2,
-             "tn_pack_layout_i64": 2}
+_LAUNCHES = {"tn_attn_prep": 3, "tn_attn_bwd_bf16": 3, "tn_attn_decode_bf16": 2, "tn_logmel_power_f32": 2,
+             "tn_rmsnorm_bwd_bf16": 2, "tn_pack_layout_i64": 2}
 launch_count = 0
 _hooks = []   # callables(name, phase) with phase in {"pre", "post"}; bench.py uses them to time kernel classes
 

@@ -1,0 +1,419 @@
+// touchnet_b200 :: autoregressive decoding - split-KV decode attention, KV-cache append, greedy token selection.
+//
+// Replaces what transformers' `generate(use_cache=True, do_sample=False, num_beams=1)` runs per new token when the
+// reference evaluates a model (touchnet/models/touch_audio/inference_touch_audio.py:170-192): the attention of one new
+// query row per sequence over the cache (hf: DynamicCache + sdpa), the cache update, and the logits processors
+// RepetitionPenaltyLogitsProcessor / NoRepeatNGramLogitsProcessor followed by argmax.
+//
+// Decode attention is memory bound (one query row per head against S cached keys), so the kernel is organised around
+// streaming K/V: grid (split, kv head, batch row); the H/KV query heads that share a kv head are the rows of ONE
+// m16n8k16 tile (GQA ratios 1..16), 4 warps each take 16 keys of every 64-key sub-block, K/V sub-blocks arrive through a
+// DEC_STAGES-deep cp.async ring.  Every split writes an fp32 partial (O unnormalised, m in the log2 domain, l); a second
+// kernel merges the splits in split order (no atomics: bit-reproducible run to run).
+#include "../../include/touchnet_b200.h"
+#include "attn_common.cuh"
+#include "host.h"
+
+namespace tn {
+
+constexpr int DEC_THREADS = 128;   // 4 warps x 16 keys of each 64-key sub-block
+constexpr int DEC_STAGES = 3;
+constexpr int DEC_SUB_TILE = ATT_SUB * ATT_HD * 2;              // 16 KB (one of K, V)
+constexpr int DEC_Q_TILE = 16 * ATT_HD * 2;                     // 4 KB
+constexpr int DEC_SMEM = DEC_Q_TILE + DEC_STAGES * 2 * DEC_SUB_TILE;
+constexpr int DEC_TARGET_CTAS = 4 * 132;   // two resident CTAs per SM, two waves over the 132 SMs of an H100 SXM
+constexpr int DEC_MAX_SPLITS = 64;
+
+// split count: a function of the shapes only (never of the current length, so a captured graph stays valid)
+static inline int decode_splits(int B, int KV, int S_cap) {
+  const int per_row = B * KV;
+  int s = (DEC_TARGET_CTAS + per_row - 1) / per_row;
+  const int max_by_len = (S_cap + ATT_SUB - 1) / ATT_SUB;
+  if (s > max_by_len) s = max_by_len;
+  if (s > DEC_MAX_SPLITS) s = DEC_MAX_SPLITS;
+  return s < 1 ? 1 : s;
+}
+
+struct DecodeParams {
+  const bf16* Q;
+  const bf16* K;
+  const bf16* V;
+  int64_t ldq, ld_tok, ld_batch;
+  const int32_t* kv_start;
+  const int32_t* kv_end;
+  float* part_o;    // [B, H, splits, 128]
+  float* part_ml;   // [B, H, splits, 2]  (m in the log2 domain, l)
+  int H, KV, S_cap, splits, chunk;
+  float scale_log2;
+};
+
+// rows [row0, row0 + 64) of K or V into a swizzled tile; rows outside [lo, hi) are zero-filled (the cache beyond the
+// written length may hold anything, and a NaN there times a zero probability would still be NaN)
+__device__ __forceinline__ void load_kv_tile(uint32_t dst, const bf16* base, int64_t ld, int row0, int lo, int hi, int tid) {
+#pragma unroll
+  for (int i = tid; i < ATT_SUB * 16; i += DEC_THREADS) {
+    const int r = i >> 4, ch = i & 15;
+    const bool ok = row0 + r >= lo && row0 + r < hi;
+    const bf16* src = base + (ok ? int64_t(row0 + r) * ld : 0) + ch * 8;
+    cp_async16(dst + tile_off(r, ch), src, ok ? 16u : 0u);
+  }
+}
+
+__global__ void __launch_bounds__(DEC_THREADS, 2) attn_decode_kernel(const DecodeParams p) {
+  extern __shared__ __align__(128) uint8_t smem[];
+  const uint32_t sb = smem_u32(smem);
+  const int split = blockIdx.x, kvh = blockIdx.y, b = blockIdx.z;
+  const int tid = int(threadIdx.x), warp = tid >> 5, lane = tid & 31;
+  const int G = p.H / p.KV;
+  const int lo = max(p.kv_start[b], split * p.chunk);
+  const int hi = min(min(p.kv_end[b], p.S_cap), (split + 1) * p.chunk);
+  float* pml = p.part_ml + ((int64_t(b) * p.H + kvh * G) * p.splits + split) * 2;
+  float* po = p.part_o + ((int64_t(b) * p.H + kvh * G) * p.splits + split) * ATT_HD;
+  if (hi <= lo) {   // nothing of this row's range in this chunk: an empty partial
+    for (int g = tid; g < G; g += DEC_THREADS) {
+      pml[int64_t(g) * p.splits * 2] = -INFINITY;
+      pml[int64_t(g) * p.splits * 2 + 1] = 0.f;
+    }
+    return;
+  }
+  const bf16* Kb = p.K + int64_t(b) * p.ld_batch + kvh * ATT_HD;
+  const bf16* Vb = p.V + int64_t(b) * p.ld_batch + kvh * ATT_HD;
+  const int kbase = lo & ~(ATT_SUB - 1);
+  const int nsub = (hi - kbase + ATT_SUB - 1) / ATT_SUB;
+  const uint32_t sQ = sb, sK0 = sb + DEC_Q_TILE, sV0 = sK0 + DEC_STAGES * DEC_SUB_TILE;
+
+  // the G query heads of this kv head are rows 0..G-1 of a 16-row tile (rows >= G zero)
+  load_tile_async<16, DEC_THREADS>(sQ, p.Q + int64_t(b) * p.ldq + int64_t(kvh) * G * ATT_HD, ATT_HD, 0, G, tid);
+  auto load_stage = [&](int i) {
+    if (i < nsub) {
+      const int st = i % DEC_STAGES, k0 = kbase + i * ATT_SUB;
+      load_kv_tile(sK0 + st * DEC_SUB_TILE, Kb, p.ld_tok, k0, lo, hi, tid);
+      load_kv_tile(sV0 + st * DEC_SUB_TILE, Vb, p.ld_tok, k0, lo, hi, tid);
+    }
+    cp_async_commit();   // empty groups keep the group count uniform
+  };
+#pragma unroll
+  for (int i = 0; i < DEC_STAGES - 1; ++i) load_stage(i);
+
+  const int cq = 2 * (lane & 3);
+  float o[16][4];
+#pragma unroll
+  for (int i = 0; i < 16; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
+  float m_a = -INFINITY, m_b = -INFINITY, l_a = 0.f, l_b = 0.f;
+  uint32_t qf[8][4];
+
+  for (int i = 0; i < nsub; ++i) {
+    cp_async_wait<DEC_STAGES - 2>();
+    __syncthreads();                         // stage i landed for every thread; stage i-1 is no longer read
+    load_stage(i + DEC_STAGES - 1);
+    if (i == 0) {
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) ldsm_a(sQ, 0, kk, qf[kk]);
+    }
+    const int st = i % DEC_STAGES;
+    const uint32_t sK = sK0 + st * DEC_SUB_TILE, sV = sV0 + st * DEC_SUB_TILE;
+    const int k0 = kbase + i * ATT_SUB + warp * 16;   // this warp's 16 keys
+
+    float s[2][4];
+#pragma unroll
+    for (int j = 0; j < 2; ++j) s[j][0] = s[j][1] = s[j][2] = s[j][3] = 0.f;
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) {
+      uint32_t bf[4];
+      ldsm_b_nk(sK, warp * 16, kk, bf);
+      mma_bf16_16816(s[0], qf[kk], bf[0], bf[1]);
+      mma_bf16_16816(s[1], qf[kk], bf[2], bf[3]);
+    }
+    float mx_a = -INFINITY, mx_b = -INFINITY;
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int key = k0 + 8 * j + cq + (e & 1);
+        const float x = (key >= lo && key < hi) ? s[j][e] * p.scale_log2 : -INFINITY;
+        s[j][e] = x;
+        if (e < 2) mx_a = fmaxf(mx_a, x); else mx_b = fmaxf(mx_b, x);
+      }
+    }
+    mx_a = quad_max(mx_a); mx_b = quad_max(mx_b);
+    const float mn_a = fmaxf(m_a, mx_a), mn_b = fmaxf(m_b, mx_b);
+    const float mu_a = mn_a == -INFINITY ? 0.f : mn_a, mu_b = mn_b == -INFINITY ? 0.f : mn_b;
+    const float al_a = fast_exp2(m_a - mu_a), al_b = fast_exp2(m_b - mu_b);
+    m_a = mn_a; m_b = mn_b;
+    l_a *= al_a; l_b *= al_b;
+#pragma unroll
+    for (int j = 0; j < 16; ++j) { o[j][0] *= al_a; o[j][1] *= al_a; o[j][2] *= al_b; o[j][3] *= al_b; }
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      s[j][0] = fast_exp2(s[j][0] - mu_a); s[j][1] = fast_exp2(s[j][1] - mu_a);
+      s[j][2] = fast_exp2(s[j][2] - mu_b); s[j][3] = fast_exp2(s[j][3] - mu_b);
+      l_a += s[j][0] + s[j][1];
+      l_b += s[j][2] + s[j][3];
+    }
+    const uint32_t a[4] = {pack_bf16x2(s[0][0], s[0][1]), pack_bf16x2(s[0][2], s[0][3]),
+                           pack_bf16x2(s[1][0], s[1][1]), pack_bf16x2(s[1][2], s[1][3])};
+#pragma unroll
+    for (int np = 0; np < 8; ++np) {
+      uint32_t bf[4];
+      ldsm_b_kn(sV, warp * 16, np, bf);
+      mma_bf16_16816(o[2 * np], a, bf[0], bf[1]);
+      mma_bf16_16816(o[2 * np + 1], a, bf[2], bf[3]);
+    }
+  }
+  cp_async_wait<0>();
+  __syncthreads();   // the ring is free: reuse it for the cross-warp merge
+
+  // ---- merge the 4 warps (fixed order) -> this split's partial ----
+  l_a = quad_sum(l_a); l_b = quad_sum(l_b);
+  float* sO = reinterpret_cast<float*>(smem + DEC_Q_TILE);        // [4 warps][16 rows][128] fp32 = 32 KB
+  float* sM = sO + 4 * 16 * ATT_HD;                               // [4][16]
+  float* sL = sM + 4 * 16;                                        // [4][16]
+  const int ra = lane >> 2;
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    const int col = 8 * j + cq;
+    float* wa = sO + (warp * 16 + ra) * ATT_HD + col;
+    float* wb = sO + (warp * 16 + ra + 8) * ATT_HD + col;
+    wa[0] = o[j][0]; wa[1] = o[j][1]; wb[0] = o[j][2]; wb[1] = o[j][3];
+  }
+  if ((lane & 3) == 0) {
+    sM[warp * 16 + ra] = m_a; sM[warp * 16 + ra + 8] = m_b;
+    sL[warp * 16 + ra] = l_a; sL[warp * 16 + ra + 8] = l_b;
+  }
+  __syncthreads();
+  for (int i = tid; i < G * ATT_HD; i += DEC_THREADS) {
+    const int g = i / ATT_HD, c = i % ATT_HD;
+    float M = -INFINITY;
+#pragma unroll
+    for (int w = 0; w < 4; ++w) M = fmaxf(M, sM[w * 16 + g]);
+    const float Mu = M == -INFINITY ? 0.f : M;
+    float acc = 0.f, L = 0.f;
+#pragma unroll
+    for (int w = 0; w < 4; ++w) {
+      const float f = fast_exp2(sM[w * 16 + g] - Mu);
+      acc += f * sO[(w * 16 + g) * ATT_HD + c];
+      L += f * sL[w * 16 + g];
+    }
+    po[int64_t(g) * p.splits * ATT_HD + c] = acc;
+    if (c == 0) {
+      pml[int64_t(g) * p.splits * 2] = M;
+      pml[int64_t(g) * p.splits * 2 + 1] = L;
+    }
+  }
+}
+
+// one CTA (128 threads = 128 columns) per (row, head): combine the splits in split order
+__global__ void __launch_bounds__(ATT_HD) attn_decode_merge_kernel(const float* __restrict__ part_o,
+                                                                   const float* __restrict__ part_ml, bf16* __restrict__ O,
+                                                                   int64_t ldo, float* __restrict__ lse, int H, int splits) {
+  const int h = blockIdx.x, b = blockIdx.y, c = threadIdx.x;
+  const float* ml = part_ml + (int64_t(b) * H + h) * splits * 2;
+  const float* po = part_o + (int64_t(b) * H + h) * splits * ATT_HD;
+  float M = -INFINITY;
+  for (int s = 0; s < splits; ++s)
+    if (ml[2 * s + 1] > 0.f) M = fmaxf(M, ml[2 * s]);
+  float acc = 0.f, L = 0.f;
+  if (M != -INFINITY) {
+    for (int s = 0; s < splits; ++s) {
+      const float l = ml[2 * s + 1];
+      if (l > 0.f) {
+        const float f = fast_exp2(ml[2 * s] - M);
+        acc += f * po[int64_t(s) * ATT_HD + c];
+        L += f * l;
+      }
+    }
+  }
+  const float inv = L > 0.f ? 1.f / L : 0.f;
+  O[int64_t(b) * ldo + int64_t(h) * ATT_HD + c] = __float2bfloat16_rn(acc * inv);
+  if (lse && c == 0) {
+    constexpr float LN2 = 0.6931471805599453f;
+    lse[int64_t(b) * H + h] = L > 0.f ? (M + __log2f(L)) * LN2 : INFINITY;
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// cache append: rows [end[b] - T_new, end[b]) of batch row b <- source rows b*T_new .. b*T_new + T_new - 1
+// ---------------------------------------------------------------------------------------------------------------
+__global__ void kv_append_kernel(const bf16* __restrict__ K, int64_t ldk, const bf16* __restrict__ V, int64_t ldv,
+                                 bf16* __restrict__ Kc, bf16* __restrict__ Vc, int64_t ld_tok, int64_t ld_batch,
+                                 const int32_t* __restrict__ row_end, int T_new, int S_cap, int width) {
+  const int t = blockIdx.x, b = blockIdx.y;
+  const int row = row_end[b] - T_new + t;
+  if (row < 0 || row >= S_cap) return;
+  const int64_t src = int64_t(b) * T_new + t;
+  const int64_t dst = int64_t(b) * ld_batch + int64_t(row) * ld_tok;
+  for (int i = threadIdx.x; i < width / 8; i += blockDim.x) {
+    reinterpret_cast<uint4*>(Kc + dst)[i] = reinterpret_cast<const uint4*>(K + src * ldk)[i];
+    reinterpret_cast<uint4*>(Vc + dst)[i] = reinterpret_cast<const uint4*>(V + src * ldv)[i];
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// greedy selection with HF's repetition penalty and no-repeat-ngram processors, one CTA per batch row
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int SEL_THREADS = 1024;
+
+// torch.argmax order: NaN above every number, then the larger value, then the lower index; index -1 = no candidate
+__device__ __forceinline__ bool argmax_better(float x, int i, float best, int bi) {
+  if (i < 0) return false;
+  if (bi < 0) return true;
+  const bool nx = x != x, nb = best != best;
+  if (nx != nb) return nx;
+  if (!nx && x != best) return x > best;
+  return i < bi;
+}
+
+__global__ void __launch_bounds__(SEL_THREADS) greedy_select_kernel(
+    const bf16* __restrict__ logits, int64_t ld, int V, int64_t* __restrict__ history, int64_t ld_hist,
+    int32_t* __restrict__ length, int64_t* __restrict__ positions, int64_t* __restrict__ next_ids,
+    int32_t* __restrict__ finished, float penalty, int ngram, int64_t eos, int64_t pad) {
+  extern __shared__ uint32_t bits[];   // [2][words]: repetition set, banned set
+  __shared__ float s_val[SEL_THREADS / 32];
+  __shared__ int s_idx[SEL_THREADS / 32];
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const int words = (V + 31) / 32;
+  uint32_t* rep = bits;
+  uint32_t* ban = bits + words;
+  for (int i = tid; i < 2 * words; i += SEL_THREADS) bits[i] = 0u;
+  __syncthreads();
+  const int len = length[b];
+  const int64_t* h = history + int64_t(b) * ld_hist;
+  const bool use_pen = penalty != 1.0f;
+  if (use_pen) {
+    for (int i = tid; i < len; i += SEL_THREADS) {
+      const int64_t id = h[i];
+      if (id >= 0 && id < V) atomicOr(&rep[id >> 5], 1u << (id & 31));
+    }
+  }
+  if (ngram > 0 && len + 1 >= ngram) {
+    // ngram i = h[i .. i+n-1]; its last id is banned when its first n-1 ids equal the last n-1 ids of the sequence
+    for (int i = tid; i + ngram <= len; i += SEL_THREADS) {
+      bool match = true;
+      for (int j = 0; j < ngram - 1 && match; ++j) match = h[i + j] == h[len - ngram + 1 + j];
+      const int64_t id = h[i + ngram - 1];
+      if (match && id >= 0 && id < V) atomicOr(&ban[id >> 5], 1u << (id & 31));
+    }
+  }
+  __syncthreads();
+  const bf16* row = logits + int64_t(b) * ld;
+  float best = -INFINITY;
+  int bi = -1;
+  for (int v = tid; v < V; v += SEL_THREADS) {   // increasing v per thread: strict '>' keeps the lowest index
+    float x = __bfloat162float(row[v]);
+    if (use_pen && (rep[v >> 5] >> (v & 31) & 1u)) x = x < 0.f ? x * penalty : x / penalty;
+    if (ban[v >> 5] >> (v & 31) & 1u) x = -INFINITY;
+    if (argmax_better(x, v, best, bi)) { best = x; bi = v; }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float ov = __shfl_xor_sync(0xffffffffu, best, o);
+    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+    if (argmax_better(ov, oi, best, bi)) { best = ov; bi = oi; }
+  }
+  if ((tid & 31) == 0) { s_val[tid >> 5] = best; s_idx[tid >> 5] = bi; }
+  __syncthreads();
+  if (tid == 0) {
+    best = s_val[0]; bi = s_idx[0];
+    for (int w = 1; w < SEL_THREADS / 32; ++w) {
+      const float ov = s_val[w];
+      const int oi = s_idx[w];
+      if (argmax_better(ov, oi, best, bi)) { best = ov; bi = oi; }
+    }
+    const int fin = finished[b];
+    const int64_t tok = fin ? pad : int64_t(bi);
+    if (len < ld_hist) history[int64_t(b) * ld_hist + len] = tok;
+    next_ids[b] = tok;
+    length[b] = len + 1;
+    positions[b] += 1;
+    if (tok == eos) finished[b] = 1;
+  }
+}
+
+}  // namespace tn
+
+using namespace tn;
+
+extern "C" int64_t tn_attn_decode_ws_floats(int B, int H, int KV, int S_cap) {
+  if (B <= 0 || H <= 0 || KV <= 0 || S_cap <= 0) return 0;
+  return int64_t(B) * H * decode_splits(B, KV, S_cap) * (ATT_HD + 2);
+}
+
+extern "C" int tn_attn_decode_bf16(const void* Q, int64_t ldq, const void* K, const void* V, int64_t ld_tok,
+                                   int64_t ld_batch, const int32_t* kv_start, const int32_t* kv_end, int B, int H, int KV,
+                                   int S_cap, float scale, float* workspace, void* O, int64_t ldo, float* lse,
+                                   tn_stream_t stream_) {
+  clear_error();
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  TN_REQUIRE(Q && K && V && kv_start && kv_end && workspace && O, "tn_attn_decode_bf16: null pointer");
+  TN_REQUIRE(B > 0 && H > 0 && KV > 0 && S_cap > 0 && H % KV == 0 && H / KV <= 16,
+             "tn_attn_decode_bf16: bad dims B=%d H=%d KV=%d S_cap=%d (H/KV must be 1..16)", B, H, KV, S_cap);
+  TN_REQUIRE(ldq % 8 == 0 && ld_tok % 8 == 0 && ld_batch % 8 == 0 && ldo % 8 == 0,
+             "tn_attn_decode_bf16: strides must be multiples of 8");
+  TN_REQUIRE(ldq >= int64_t(H) * ATT_HD && ldo >= int64_t(H) * ATT_HD && ld_tok >= int64_t(KV) * ATT_HD &&
+                 ld_batch >= ld_tok * S_cap, "tn_attn_decode_bf16: stride smaller than the rows it must hold");
+  const int splits = decode_splits(B, KV, S_cap);
+  DecodeParams p{};
+  p.Q = static_cast<const bf16*>(Q); p.K = static_cast<const bf16*>(K); p.V = static_cast<const bf16*>(V);
+  p.ldq = ldq; p.ld_tok = ld_tok; p.ld_batch = ld_batch;
+  p.kv_start = kv_start; p.kv_end = kv_end;
+  p.part_o = workspace;
+  p.part_ml = workspace + int64_t(B) * H * splits * ATT_HD;
+  p.H = H; p.KV = KV; p.S_cap = S_cap; p.splits = splits;
+  p.chunk = ((S_cap + splits - 1) / splits + ATT_SUB - 1) / ATT_SUB * ATT_SUB;
+  p.scale_log2 = scale * 1.4426950408889634f;
+  static bool configured = false;
+  if (!configured) {
+    TN_CHECK_CUDA(cudaFuncSetAttribute(attn_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DEC_SMEM));
+    configured = true;
+  }
+  attn_decode_kernel<<<dim3(splits, KV, B), DEC_THREADS, DEC_SMEM, stream>>>(p);
+  TN_CHECK_CUDA(cudaGetLastError());
+  attn_decode_merge_kernel<<<dim3(H, B), ATT_HD, 0, stream>>>(p.part_o, p.part_ml, static_cast<bf16*>(O), ldo, lse, H,
+                                                              splits);
+  TN_CHECK_CUDA(cudaGetLastError());
+  return TN_OK;
+}
+
+extern "C" int tn_kv_append_bf16(const void* K, int64_t ldk, const void* V, int64_t ldv, void* K_cache, void* V_cache,
+                                 int64_t ld_tok, int64_t ld_batch, const int32_t* row_end, int B, int T_new, int S_cap,
+                                 int width, tn_stream_t stream_) {
+  clear_error();
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  TN_REQUIRE(K && V && K_cache && V_cache && row_end, "tn_kv_append_bf16: null pointer");
+  TN_REQUIRE(B > 0 && T_new > 0 && S_cap >= T_new && width > 0 && width % 8 == 0,
+             "tn_kv_append_bf16: bad dims B=%d T_new=%d S_cap=%d width=%d", B, T_new, S_cap, width);
+  TN_REQUIRE(ldk % 8 == 0 && ldv % 8 == 0 && ld_tok % 8 == 0 && ld_batch % 8 == 0 && ldk >= width && ldv >= width &&
+                 ld_tok >= width && ld_batch >= ld_tok * S_cap, "tn_kv_append_bf16: bad strides");
+  TN_REQUIRE(T_new <= 65535 && B <= 65535, "tn_kv_append_bf16: grid too large");
+  TN_REQUIRE(((uintptr_t(K) | uintptr_t(V) | uintptr_t(K_cache) | uintptr_t(V_cache)) & 15) == 0,
+             "tn_kv_append_bf16: pointers must be 16-byte aligned");
+  kv_append_kernel<<<dim3(T_new, B), 128, 0, stream>>>(
+      static_cast<const bf16*>(K), ldk, static_cast<const bf16*>(V), ldv, static_cast<bf16*>(K_cache),
+      static_cast<bf16*>(V_cache), ld_tok, ld_batch, row_end, T_new, S_cap, width);
+  TN_CHECK_CUDA(cudaGetLastError());
+  return TN_OK;
+}
+
+extern "C" int tn_greedy_select_bf16(const void* logits, int64_t ld, int B, int V, int64_t* history, int64_t ld_hist,
+                                     int32_t* length, int64_t* positions, int64_t* next_ids, int32_t* finished,
+                                     float repetition_penalty, int no_repeat_ngram_size, int64_t eos, int64_t pad,
+                                     tn_stream_t stream_) {
+  clear_error();
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  TN_REQUIRE(logits && history && length && positions && next_ids && finished, "tn_greedy_select_bf16: null pointer");
+  TN_REQUIRE(B > 0 && V > 0 && ld >= V && ld_hist > 0, "tn_greedy_select_bf16: bad dims B=%d V=%d", B, V);
+  TN_REQUIRE(repetition_penalty > 0.f, "tn_greedy_select_bf16: repetition_penalty must be > 0");
+  TN_REQUIRE(no_repeat_ngram_size >= 0, "tn_greedy_select_bf16: no_repeat_ngram_size must be >= 0");
+  const size_t smem = size_t(2) * ((V + 31) / 32) * sizeof(uint32_t);
+  TN_REQUIRE(smem <= 200 * 1024, "tn_greedy_select_bf16: vocabulary of %d too large for the shared-memory bitmaps", V);
+  static bool configured = false;
+  if (!configured) {
+    TN_CHECK_CUDA(cudaFuncSetAttribute(greedy_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    configured = true;
+  }
+  greedy_select_kernel<<<B, SEL_THREADS, smem, stream>>>(static_cast<const bf16*>(logits), ld, V, history, ld_hist,
+                                                         length, positions, next_ids, finished, repetition_penalty,
+                                                         no_repeat_ngram_size, eos, pad);
+  TN_CHECK_CUDA(cudaGetLastError());
+  return TN_OK;
+}

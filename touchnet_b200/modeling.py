@@ -346,6 +346,10 @@ class B200LlamaForCausalLM(nn.Module):
                 position_ids: Optional[torch.Tensor] = None, past_key_values=None,
                 inputs_embeds: Optional[torch.Tensor] = None, labels=None, use_cache=None, **kwargs: Any):
         assert labels is None, "loss is computed in the train loop (ref: modeling_touch_audio.py:121)"
+        if past_key_values is not None and use_cache is not False:
+            from . import generation
+            if isinstance(past_key_values, generation.B200KVCache):    # prefill or one decode step (generation.py)
+                return generation.forward_cached(self, past_key_values, input_ids, None, attention_mask, position_ids)
         ops.begin_forward(self)             # side-stream casts of stale fp32 master weights / new cache epoch under FSDP2
         tp_group = getattr(self, "tp_group", None)
         if inputs_embeds is None:
@@ -387,6 +391,15 @@ class B200LlamaForCausalLM(nn.Module):
                 logits = tensor_parallel.lm_head(h, self.lm_head.weight, tpc)
         out = CausalLMOutputWithPast(logits=logits)
         return out
+
+    def generate(self, input_ids: torch.Tensor, attention_mask: Optional[torch.Tensor] = None,
+                 position_ids: Optional[torch.Tensor] = None, **kwargs: Any) -> torch.Tensor:
+        """Greedy decoding with a KV cache, HF `generate` semantics (see generation.generate)."""
+        from . import generation
+        if kwargs.get("input_features") is not None:
+            raise TouchNetB200Error("generate: unsupported arguments ['input_features'] (a text-only model)")
+        kwargs.pop("input_features", None)
+        return generation.generate(self, input_ids, None, attention_mask, position_ids, **kwargs)
 
 
 class B200TouchAudioForCausalLM(nn.Module):
@@ -463,6 +476,11 @@ class B200TouchAudioForCausalLM(nn.Module):
                 output_attentions=None, output_hidden_states=None, return_dict=None, cache_position=None,
                 logits_to_keep=0, check_nan: bool = True, **kwargs: Any):
         assert labels is None  # we calculate loss in train-loop (ref: modeling_touch_audio.py:121)
+        if past_key_values is not None and use_cache is not False:
+            from . import generation
+            if isinstance(past_key_values, generation.B200KVCache):    # prefill or one decode step (generation.py)
+                return generation.forward_cached(self, past_key_values, input_ids, input_features, attention_mask,
+                                                 position_ids)
         ops.begin_forward(self)             # projector, decoder layers, lm_head: casts overlap the GEMMs in front of them
         tp_group = getattr(self, "tp_group", None)
         if inputs_embeds is None and tp_group is not None:
@@ -493,6 +511,14 @@ class B200TouchAudioForCausalLM(nn.Module):
                                       inputs_embeds=inputs_embeds, **kwargs)
         outputs.attention_mask = attention_mask
         return outputs
+
+    def generate(self, input_ids: torch.Tensor, input_features: Optional[torch.Tensor] = None,
+                 attention_mask: Optional[torch.Tensor] = None, position_ids: Optional[torch.Tensor] = None,
+                 **kwargs: Any) -> torch.Tensor:
+        """The reference's evaluation call (ref: inference_touch_audio.py:170-192): greedy decoding with a KV cache, HF
+        `generate` semantics, the audio features projected into the prompt only (see generation.generate)."""
+        from . import generation
+        return generation.generate(self, input_ids, input_features, attention_mask, position_ids, **kwargs)
 
 
 __all__ = ["B200LlamaForCausalLM", "B200TouchAudioForCausalLM", "B200LlamaModel", "B200DecoderLayer", "B200RMSNorm",

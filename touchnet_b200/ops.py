@@ -379,6 +379,48 @@ def attn_bwd(q, k, v, o, do, lse, plan: AttnPlan, H: int, KV: int, scale: float,
     return dq, dk, dv
 
 
+def attn_decode(q, k_cache, v_cache, kv_start, kv_end, H: int, KV: int, scale: float, workspace=None, lse: bool = False):
+    """Split-KV attention of one query row per batch row: q [B, H*128] (rotated) against cache rows [kv_start[b],
+    kv_end[b]) of k_cache / v_cache [B, S_cap, KV*128] (token and batch strides shared by both) -> o [B, H*128]
+    (and lse [B, H] if asked)."""
+    _chk(q, "q", BF16); _chk(k_cache, "k_cache", BF16); _chk(v_cache, "v_cache", BF16)
+    B, S_cap = k_cache.shape[0], k_cache.shape[1]
+    assert k_cache.stride() == v_cache.stride() and k_cache.stride(2) == 1 and q.stride(1) == 1
+    if workspace is None:
+        workspace = torch.empty(int(_lib.load().tn_attn_decode_ws_floats(B, H, KV, S_cap)), dtype=torch.float32,
+                                device=q.device)
+    o = torch.empty((B, H * 128), dtype=BF16, device=q.device)
+    lse_t = torch.empty((B, H), dtype=torch.float32, device=q.device) if lse else None
+    _lib.call("tn_attn_decode_bf16", q.data_ptr(), q.stride(0), k_cache.data_ptr(), v_cache.data_ptr(),
+              k_cache.stride(1), k_cache.stride(0), kv_start.data_ptr(), kv_end.data_ptr(), B, H, KV, S_cap, float(scale),
+              workspace.data_ptr(), o.data_ptr(), o.stride(0), None if lse_t is None else lse_t.data_ptr(), _st())
+    return (o, lse_t) if lse else o
+
+
+def kv_append(k, v, k_cache, v_cache, row_end, T_new: int):
+    """Cache rows [row_end[b] - T_new, row_end[b]) of batch row b <- rows b*T_new .. of k / v [B*T_new, KV*128]."""
+    _chk(k, "k", BF16); _chk(v, "v", BF16); _chk(k_cache, "k_cache", BF16); _chk(row_end, "row_end", torch.int32)
+    B, S_cap, width = k_cache.shape
+    assert k_cache.stride() == v_cache.stride() and k.shape[1] == width and k.stride(1) == 1 and v.stride(1) == 1
+    _lib.call("tn_kv_append_bf16", k.data_ptr(), k.stride(0), v.data_ptr(), v.stride(0), k_cache.data_ptr(),
+              v_cache.data_ptr(), k_cache.stride(1), k_cache.stride(0), row_end.data_ptr(), B, int(T_new), S_cap, width,
+              _st())
+
+
+def greedy_select(logits, history, length, positions, next_ids, finished, repetition_penalty: float,
+                  no_repeat_ngram_size: int, eos: int, pad: int):
+    """Greedy next token of every row (HF repetition penalty + no-repeat-ngram + argmax on fp32-cast bf16 logits [B, V]),
+    written into history / next_ids; advances length and positions, updates finished (all device tensors, in place)."""
+    _chk(logits, "logits", BF16); _chk(history, "history", torch.int64); _chk(length, "length", torch.int32)
+    _chk(positions, "positions", torch.int64); _chk(next_ids, "next_ids", torch.int64)
+    _chk(finished, "finished", torch.int32)
+    B, V = logits.shape
+    assert logits.stride(1) == 1 and history.stride(1) == 1 and history.shape[0] == B
+    _lib.call("tn_greedy_select_bf16", logits.data_ptr(), logits.stride(0), B, V, history.data_ptr(), history.stride(0),
+              length.data_ptr(), positions.data_ptr(), next_ids.data_ptr(), finished.data_ptr(),
+              float(repetition_penalty), int(no_repeat_ngram_size), int(eos), int(pad), _st())
+
+
 def embed_add(input_ids: Optional[torch.Tensor], embed: Optional[torch.Tensor], proj: Optional[torch.Tensor],
               rows: int, d: int, nan_flag: Optional[torch.Tensor] = None):
     """E = embed[input_ids] + proj (either may be None)."""
@@ -541,6 +583,45 @@ def _unpad_heads(x: torch.Tensor, heads: int, hd: int) -> torch.Tensor:
     return x.view(x.shape[0], heads, 128)[:, :, :hd].reshape(x.shape[0], heads * hd)
 
 
+def block_forward(x2, ln1, wqb, wkb, wvb, bq, bk, bv, wob, ln2, wgb, wub, wdb, cos, sin, H, KV, eps, hd, attend, tp=None,
+                  need_gu=True):
+    """Forward of one pre-norm decoder block on rows x2 [M, d] with bf16 working weights - the body shared by training
+    (DecoderLayerFn), prompt prefill and cached decoding (generation.py), which differ only in `attend(q, k, v) ->
+    (o, lse, k, v)`: q/k/v arrive projected, rotated and (head_dim < 128) zero-padded to 128-wide heads.
+    Returns (out, saved) with saved = (rstd1, h1, q, k, v, o, lse, x1, rstd2, h2, g, u, hm) for the backward."""
+    h1, _, rstd1 = rmsnorm_fwd(x2, ln1, eps)
+    if tp is not None:
+        h1 = tp.gather_rows(h1, keep=True)                               # [B*T, d]: every row, for the local heads
+    nq, nkv = wqb.shape[0], wkb.shape[0]
+    rope_in_gemm = qkv_fusable(h1.shape[0], nq, nkv) and bq is None and hd == 128   # RoPE in the QKV GEMM epilogue
+    if qkv_fusable(h1.shape[0], nq, nkv):
+        qkv = gemm_qkv_fwd(h1, wqb, wkb, wvb, rope=(cos, sin) if rope_in_gemm else None)
+        q, k, v = qkv[:, :nq], qkv[:, nq:nq + nkv], qkv[:, nq + nkv:]
+    else:
+        q = gemm(h1, wqb); k = gemm(h1, wkb); v = gemm(h1, wvb)
+    if bq is not None:
+        q += bq.to(BF16); k += bk.to(BF16); v += bv.to(BF16)
+    if not rope_in_gemm:
+        rope_apply_(q, cos, sin, H, hd)
+        rope_apply_(k, cos, sin, KV, hd)
+    if hd != 128:      # head_dim 64 (Llama-3.2-1B, the reference's example config) etc.: zero-padded heads, 128-wide kernels
+        q, k, v = _pad_heads(q, H, hd), _pad_heads(k, KV, hd), _pad_heads(v, KV, hd)
+    o, lse, k, v = attend(q, k, v)
+    if tp is None:
+        x1 = gemm(o if hd == 128 else _unpad_heads(o, H, hd), wob, residual=x2)
+    else:                                                                # partial sums over tp -> this rank's rows
+        x1 = tp.gemm_reduce_scatter(o, wob, x2)
+    h2, _, rstd2 = rmsnorm_fwd(x1, ln2, eps)
+    if tp is not None:
+        h2 = tp.gather_rows(h2, keep=True)
+    g, u, hm = gemm_swiglu(h2, wgb, wub, need_gu)
+    if tp is None:
+        out = gemm(hm, wdb, residual=x1)
+    else:
+        out = tp.gemm_reduce_scatter(hm, wdb, x1)
+    return out, (rstd1, h1, q, k, v, o, lse, x1, rstd2, h2, g, u, hm)
+
+
 class DecoderLayerFn(torch.autograd.Function):
     """One pre-norm decoder block as a single autograd node (hf: LlamaDecoderLayer.forward modeling_llama.py:303-333):
     7 kernel launches forward, residual adds fused into the o_proj / down_proj GEMM epilogues, q/k/v projections one
@@ -559,40 +640,18 @@ class DecoderLayerFn(torch.autograd.Function):
         tp = plan.tp                # tensor + sequence parallel: x holds T/tp rows, weights are this rank's shards
         if tp is not None and plan.cp_group is not None:
             raise _lib.TouchNetB200Error("tensor parallelism and context parallelism cannot be combined in one block")
-        h1, _, rstd1 = rmsnorm_fwd(x2, ln1, eps)
-        if tp is not None:
-            h1 = tp.gather_rows(h1, keep=True)                               # [B*T, d]: every row, for the local heads
-        nq, nkv = wq.shape[0], wk.shape[0]
-        rope_in_gemm = qkv_fusable(h1.shape[0], nq, nkv) and bq is None and hd == 128   # RoPE in the QKV GEMM epilogue
-        if qkv_fusable(h1.shape[0], nq, nkv):
-            qkv = gemm_qkv_fwd(h1, wqb, wkb, wvb, rope=(cos, sin) if rope_in_gemm else None)
-            q, k, v = qkv[:, :nq], qkv[:, nq:nq + nkv], qkv[:, nq + nkv:]
-        else:
-            q = gemm(h1, wqb); k = gemm(h1, wkb); v = gemm(h1, wvb)
-        if bq is not None:
-            q += bq.to(BF16); k += bk.to(BF16); v += bv.to(BF16)
-        if not rope_in_gemm:
-            rope_apply_(q, cos, sin, H, hd)
-            rope_apply_(k, cos, sin, KV, hd)
-        if hd != 128:      # head_dim 64 (Llama-3.2-1B, the reference's example config) etc.: zero-padded heads, 128-wide kernels
-            q, k, v = _pad_heads(q, H, hd), _pad_heads(k, KV, hd), _pad_heads(v, KV, hd)
-        if plan.cp_group is None:
-            o, lse = attn_fwd(q, k, v, plan, H, KV, scale)
-        else:   # context parallel: K/V of all cp ranks are gathered, the kernel runs on this rank's query window
+
+        def attend(q, k, v):
+            if plan.cp_group is None:
+                o, lse = attn_fwd(q, k, v, plan, H, KV, scale)
+                return o, lse, k, v
+            # context parallel: K/V of all cp ranks are gathered, the kernel runs on this rank's query window
             from . import context_parallel as _cp
-            o, lse, k, v = _cp.cp_attn_fwd(q, k, v, plan, H, KV, scale)
-        if tp is None:
-            x1 = gemm(o if hd == 128 else _unpad_heads(o, H, hd), wob, residual=x2)
-        else:                                                                # partial sums over tp -> this rank's rows
-            x1 = tp.gemm_reduce_scatter(o, wob, x2)
-        h2, _, rstd2 = rmsnorm_fwd(x1, ln2, eps)
-        if tp is not None:
-            h2 = tp.gather_rows(h2, keep=True)
-        g, u, hm = gemm_swiglu(h2, wgb, wub)
-        if tp is None:
-            out = gemm(hm, wdb, residual=x1)
-        else:
-            out = tp.gemm_reduce_scatter(hm, wdb, x1)
+            return _cp.cp_attn_fwd(q, k, v, plan, H, KV, scale)
+
+        out, saved = block_forward(x2, ln1, wqb, wkb, wvb, bq, bk, bv, wob, ln2, wgb, wub, wdb, cos, sin, H, KV, eps, hd,
+                                   attend, tp)
+        rstd1, h1, q, k, v, o, lse, x1, rstd2, h2, g, u, hm = saved
         ctx.save_for_backward(x2, ln1, ln2, wqb, wkb, wvb, wob, wgb, wub, wdb, cos, sin, rstd1, h1, q, k, v, o, lse, x1,
                               rstd2, h2, g, u, hm)
         ctx.plan, ctx.H, ctx.KV, ctx.scale, ctx.has_bias, ctx.hd = plan, H, KV, scale, bq is not None, hd
