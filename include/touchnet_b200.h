@@ -199,6 +199,31 @@ int tn_feat_stack_f32(const float* feats, const int64_t* frame_offsets, const in
                       const int64_t* dst_row0, int64_t out_ld, tn_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
+ * Data augmentation of the ASR recipe (touchnet/data/functions.py:83-114 audio_resample / audio_speed_perturb and
+ * :193-255 audiofeat_spec_aug / audiofeat_spec_sub / audiofeat_spec_trim), applied to utterances packed back to back.
+ * The random draws are made on the host in the reference's order (touchnet_b200/augment.py); these apply them.
+ *   tn_resample_f32: polyphase FIR of torchaudio.transforms.Resample.  Utterance u uses bank_table[utt_bank[u]] =
+ *     (orig, new, width, taps, offset) - gcd-reduced rates, filter half-width, taps = 2*width + orig, offset of its
+ *     [new, taps] fp32 bank in `banks` - and writes y[i*new + j] = sum_k w[j][k] * x[i*orig - width + k] for its
+ *     out_offsets[u+1] - out_offsets[u] outputs (x is zero outside the utterance).  x is fp32 or int16 (scaled by
+ *     2^-15).  A (1, 1) bank is an exact copy.  Speed perturbation s at rate sr is the bank (sr*s -> sr).
+ *     bank_table is a HOST array of n_banks <= 16 rows; tile_offsets[u] = first tile of utterance u, tile = output
+ *     samples per tile (multiple of 32).  Fixed summation order: bit-reproducible.
+ *   tn_spec_augment_f32: out of place.  Output frame f of utterance u (frames in_frame_offsets -> out_frame_offsets,
+ *     the output already trimmed) = input frame f - pos of the last sub (start, end, pos) with start <= f < end, else
+ *     f; zero if that source frame lies in a time mask [start, end) or the column in a frequency mask.  Tables are per
+ *     utterance, fixed width: t_masks [n_utts][n_t_masks][2], f_masks [n_utts][n_f_masks][2], subs
+ *     [n_utts][n_subs][3] int32 (empty entries: start == end).
+ */
+int tn_resample_f32(const void* x, int x_is_i16, const int64_t* in_offsets, const int64_t* out_offsets,
+                    const int64_t* tile_offsets, const int32_t* utt_bank, int n_utts, int64_t n_tiles, int tile,
+                    const int32_t* bank_table, int n_banks, const float* banks, float* y, tn_stream_t stream);
+int tn_spec_augment_f32(const float* in, const int64_t* in_frame_offsets, const int64_t* out_frame_offsets, int n_utts,
+                        int64_t total_out_frames, int n_feat, const int32_t* t_masks, int n_t_masks,
+                        const int32_t* f_masks, int n_f_masks, const int32_t* subs, int n_subs, float* out,
+                        tn_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------------------------
  * Small fused elementwise helpers on the path.
  *   tn_embed_add: E = embed[input_ids] + P   (touchnet/models/touch_audio/modeling_touch_audio.py:124-131), with the
  *     NaN check of :133-134 folded in (nan_flag[0] set to 1 if any NaN; read lazily by the caller, no sync here).

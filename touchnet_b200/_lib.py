@@ -48,6 +48,8 @@ _SIGNATURES = {
     "tn_logmel_power_f32": [_vp, _vp, _vp, _i, _i64, _i, _i, _vp, _vp, _i, _vp, _vp, _vp],
     "tn_logmel_finish_f32": [_vp, _vp, _vp, _i, _i64, _i, _vp],
     "tn_feat_stack_f32": [_vp, _vp, _vp, _i, _i64, _i, _i, _i, _i, _vp, _vp, _i64, _vp],
+    "tn_resample_f32": [_vp, _i, _vp, _vp, _vp, _vp, _i, _i64, _i, _vp, _i, _vp, _vp, _vp],
+    "tn_spec_augment_f32": [_vp, _vp, _vp, _i, _i64, _i, _vp, _i, _vp, _i, _vp, _i, _vp, _vp],
     "tn_embed_add_bf16": [_vp, _vp, _i, _vp, _vp, _vp, _i64, _i, _i64, _vp],
     "tn_cast_f32_bf16": [_vp, _vp, _i64, _vp],
     "tn_bestrq_tokenize_f32": [_vp, _i64, _vp, _vp, _i64, _i, _i, _i, _vp, _vp],

@@ -8,22 +8,31 @@ argument meaning and dict keys:
     audio_compute_log_mel_spectrogram   ref: touchnet/data/functions.py:159-190
     audiofeat_stack                     ref: touchnet/data/functions.py:258-286
 
-plus batch-level entry points (`fbank_batch`, `log_mel_batch`, `stack_batch`, `fbank_stack_batch`) that featurise a
-whole packed batch of utterances in one launch each - the form used after the H2D copy in the train step
-(SURVEY 8(b) "data-frontend boundary", option (i)).  All arithmetic happens in libtouchnet_b200.so
-(csrc/frontend.cu); windows and mel filter banks are small constants built once on the host exactly as the reference's
-third-party code builds them and cached per device.
+and the recipe's augmentation stages (draws as the reference makes them, application on the GPU, csrc/augment.cu):
+
+    audio_resample                      ref: touchnet/data/functions.py:83-96
+    audio_speed_perturb                 ref: touchnet/data/functions.py:99-114
+    audiofeat_spec_aug / _sub / _trim   ref: touchnet/data/functions.py:193-255
+
+plus batch-level entry points (`fbank_batch`, `log_mel_batch`, `stack_batch`, `fbank_stack_batch`, `resample_batch`,
+`speed_perturb_batch`, `spec_augment_batch`, `augmented_fbank_stack_batch`) that process a whole packed batch of
+utterances in one launch each - the form used after the H2D copy in the train step (SURVEY 8(b) "data-frontend
+boundary", option (i)); for augmentation, the records come from augment.draw_stage in the DataLoader worker.  All
+arithmetic happens in libtouchnet_b200.so (csrc/frontend.cu, csrc/augment.cu); windows, mel filter banks and resampling
+banks are small constants built once on the host exactly as the reference's third-party code builds them and cached per
+device.
 """
 from __future__ import annotations
 
 import math
+import random
 from functools import lru_cache
 from typing import Iterable, Iterator, Sequence
 
 import numpy as np
 import torch
 
-from . import _lib
+from . import _lib, augment
 
 MILLISECONDS_TO_SECONDS = 0.001
 
@@ -197,6 +206,130 @@ def fbank_stack_batch(wav: torch.Tensor, lens: Sequence[int], *, sample_rate=160
 
 
 # ---------------------------------------------------------------------------------------------------------------
+# augmentation (draws: augment.py; application: csrc/augment.cu)
+# ---------------------------------------------------------------------------------------------------------------
+RESAMPLE_TILE = 1024      # output samples per CTA of tn_resample_f32
+
+
+def _resample_pairs(wav: torch.Tensor, lens: Sequence[int], pairs: Sequence[tuple[int, int] | None]):
+    """Resample utterance i from pairs[i] = (orig, new) (None: exact copy) in one launch.  Returns (fp32 out, lens)."""
+    if not wav.is_cuda:
+        raise _lib.TouchNetB200Error("resampling needs the packed waveform on the GPU (no CPU path)")
+    if wav.dtype not in (torch.float32, torch.int16) or wav.dim() != 1:
+        raise _lib.TouchNetB200Error("resampling takes a 1-D packed fp32 or int16 waveform")
+    if len(pairs) != len(lens):
+        raise _lib.TouchNetB200Error(f"{len(lens)} utterances but {len(pairs)} rate pairs")
+    dev = str(wav.device)
+    keys, table, banks, utt_bank, bank_off = {}, [], [], [], 0
+    out_lens = []
+    for n, pr in zip(lens, pairs):
+        key = (1, 1) if pr is None or int(pr[0]) == int(pr[1]) else augment.reduced_ratio(*pr)
+        if pr is not None and (int(pr[0]) <= 0 or int(pr[1]) <= 0):
+            raise _lib.TouchNetB200Error(f"resampling rates must be positive, got {pr}")
+        if key not in keys:
+            keys[key] = len(table)
+            if key == (1, 1):
+                table.append((1, 1, 0, 1, 0))
+            else:
+                bank, width = augment.sinc_resample_bank(key[0], key[1], dev)
+                table.append((key[0], key[1], width, bank.shape[1], bank_off))
+                banks.append(bank.reshape(-1))
+                bank_off += bank.numel()
+        utt_bank.append(keys[key])
+        out_lens.append(int(n) if key == (1, 1) else augment.resampled_length(int(n), key[0], key[1]))
+    if len(table) > 16:
+        raise _lib.TouchNetB200Error(f"one resampling launch takes at most 16 distinct rate ratios, got {len(table)}")
+    out = torch.empty(int(sum(out_lens)), dtype=torch.float32, device=wav.device)
+    tiles = [(m + RESAMPLE_TILE - 1) // RESAMPLE_TILE for m in out_lens]
+    n_tiles = int(sum(tiles))
+    if n_tiles == 0:
+        return out, out_lens
+    meta = np.zeros((3, len(lens) + 1), dtype=np.int64)
+    for r, v in enumerate((lens, out_lens, tiles)):
+        np.cumsum(np.asarray(v, dtype=np.int64), out=meta[r, 1:])
+    meta_d = torch.from_numpy(meta).to(wav.device, non_blocking=True)
+    utt_bank_d = torch.tensor(utt_bank, dtype=torch.int32).to(wav.device, non_blocking=True)
+    table_h = np.ascontiguousarray(np.asarray(table, dtype=np.int32))
+    banks_d = torch.cat(banks) if banks else torch.zeros(1, dtype=torch.float32, device=wav.device)
+    _lib.call("tn_resample_f32", wav.data_ptr(), int(wav.dtype == torch.int16), meta_d[0].data_ptr(),
+              meta_d[1].data_ptr(), meta_d[2].data_ptr(), utt_bank_d.data_ptr(), len(lens), n_tiles, RESAMPLE_TILE,
+              table_h.ctypes.data, len(table), banks_d.data_ptr(), out.data_ptr(), _st())
+    return out, out_lens
+
+
+def resample_batch(wav: torch.Tensor, lens: Sequence[int], orig_freqs, new_freq: int):
+    """torchaudio.transforms.Resample(orig, new_freq) per utterance (ref: functions.py:83-96), one launch for the packed
+    batch.  orig_freqs: one rate or one per utterance; an utterance already at new_freq is copied exactly.
+    Returns (fp32 out, out_lens)."""
+    origs = [int(orig_freqs)] * len(lens) if np.isscalar(orig_freqs) else [int(o) for o in orig_freqs]
+    return _resample_pairs(wav, lens, [(o, int(new_freq)) for o in origs])
+
+
+def speed_perturb_batch(wav: torch.Tensor, lens: Sequence[int], speeds: Sequence[float], sample_rate: int):
+    """Speed perturbation per utterance (ref: functions.py:99-114): sox `speed s` + `rate sr` is resampling from sr*s to
+    sr, here with torchaudio's sinc filter (not sox's).  Speed 1.0 copies.  Returns (fp32 out, out_lens)."""
+    pairs = [None if float(s) == 1.0 else (augment.speed_source_rate(int(sample_rate), s), int(sample_rate))
+             for s in speeds]
+    return _resample_pairs(wav, lens, pairs)
+
+
+def spec_augment_batch(feats: torch.Tensor, frames: Sequence[int], records: Sequence[dict]):
+    """SpecAugment time/frequency masks, SpecSub and SpecTrim of augment.draw_record records (ref: functions.py:193-255),
+    out of place, one launch.  Returns (out [sum(frames_i - trim_i), F], out_frames).  Bit-exact (copies and zeros)."""
+    if not (feats.is_cuda and feats.dtype == torch.float32 and feats.dim() == 2 and feats.is_contiguous()):
+        raise _lib.TouchNetB200Error("spec_augment_batch takes contiguous [frames, F] fp32 features on the GPU")
+    if len(records) != len(frames):
+        raise _lib.TouchNetB200Error(f"{len(frames)} utterances but {len(records)} records")
+    out_frames = []
+    for t, r in zip(frames, records):
+        if r["trim"] < 0 or r["trim"] > t:
+            raise _lib.TouchNetB200Error(f"trim {r['trim']} out of range for {t} frames")
+        out_frames.append(int(t) - int(r["trim"]))
+    total = int(sum(out_frames))
+    out = torch.empty((total, feats.shape[1]), dtype=torch.float32, device=feats.device)
+    if total == 0:
+        return out, out_frames
+
+    def table(key, width):
+        n = max(len(r[key]) for r in records)
+        tab = np.zeros((len(records), max(n, 1), width), dtype=np.int32)   # empty entries: start == end == 0
+        for i, r in enumerate(records):
+            if r[key]:
+                tab[i, :len(r[key])] = np.asarray(r[key], dtype=np.int32).reshape(-1, width)
+        return torch.from_numpy(tab).to(feats.device, non_blocking=True), n
+
+    tm, n_t = table("t_masks", 2)
+    fm, n_f = table("f_masks", 2)
+    sb, n_s = table("subs", 3)
+    in_off, out_off = _offsets(frames, feats.device), _offsets(out_frames, feats.device)
+    _lib.call("tn_spec_augment_f32", feats.data_ptr(), in_off.data_ptr(), out_off.data_ptr(), len(frames), total,
+              feats.shape[1], tm.data_ptr(), n_t, fm.data_ptr(), n_f, sb.data_ptr(), n_s, out.data_ptr(), _st())
+    return out, out_frames
+
+
+def augmented_fbank_stack_batch(wav: torch.Tensor, lens: Sequence[int], records: Sequence[dict], *, sample_rate=16000,
+                                num_mel_bins=80, frame_length=25.0, frame_shift=10.0, stack_length=5, stride_length=4,
+                                normalize=True, into: torch.Tensor | None = None, dst_rows: Sequence[int] | None = None):
+    """The recipe's chain resample -> speed perturb -> fbank -> SpecAugment -> SpecSub -> SpecTrim -> stack on a packed
+    batch of raw waveforms (fp32 or int16), applying the host-drawn records of augment.draw_record / draw_stage.
+    sample_rate is the rate features are computed at (the records' resampling target).  Stages no utterance needs are
+    skipped, so with every augmentation off this is exactly fbank_batch + stack_batch.  Returns stack_batch's result."""
+    if len(records) != len(lens):
+        raise _lib.TouchNetB200Error(f"{len(lens)} utterances but {len(records)} records")
+    for r in records:
+        if r["resample"] is not None and int(r["resample"][1]) != int(sample_rate):
+            raise _lib.TouchNetB200Error(f"record resamples to {r['resample'][1]} Hz but features run at {sample_rate}")
+    if any(r["resample"] is not None for r in records):
+        wav, lens = _resample_pairs(wav, lens, [r["resample"] for r in records])
+    if any(float(r["speed"]) != 1.0 for r in records):
+        wav, lens = speed_perturb_batch(wav, lens, [r["speed"] for r in records], sample_rate)
+    feats, frames = fbank_batch(wav, lens, sample_rate, num_mel_bins, frame_length, frame_shift)
+    if any(augment.record_has_feature_ops(r) for r in records):
+        feats, frames = spec_augment_batch(feats, frames, records)
+    return stack_batch(feats, frames, stack_length, stride_length, normalize, into=into, dst_rows=dst_rows)
+
+
+# ---------------------------------------------------------------------------------------------------------------
 # per-sample generator stages (the reference's operator interface)
 # ---------------------------------------------------------------------------------------------------------------
 def _device(config) -> torch.device:
@@ -245,3 +378,75 @@ def audiofeat_stack(data: Iterable[dict], config) -> Iterator[dict]:
                              config.audiofeat_stride_length, config.audiofeat_normalize)
         sample["audiofeat"] = out
         yield sample
+
+
+def _one_utt_record(**ops) -> dict:
+    rec = {"resample": None, "speed": 1.0, "t_masks": [], "f_masks": [], "subs": [], "trim": 0}
+    rec.update(ops)
+    return rec
+
+
+def _apply_feature_ops(sample: dict, config, **ops) -> dict:
+    x = sample["audiofeat"]
+    if not x.is_cuda:
+        x = x.to(_device(config))
+    out, _ = spec_augment_batch(x.float().contiguous(), [x.shape[0]], [_one_utt_record(**ops)])
+    sample["audiofeat"] = out
+    return sample
+
+
+def audio_resample(data: Iterable[dict], config) -> Iterator[dict]:
+    """Resample to config.audio_resample_rate.  Same contract as ref: touchnet/data/functions.py:83-96 (torchaudio's
+    sinc_interp_hann filter); the waveform comes back [1, T] fp32 on the frontend device."""
+    for sample in data:
+        assert "sample_rate" in sample
+        assert "waveform" in sample
+        sample_rate = sample["sample_rate"]
+        if sample_rate != config.audio_resample_rate:
+            wav, lens = _pack([sample["waveform"]], _device(config))
+            out, _ = resample_batch(wav if wav.dtype in (torch.float32, torch.int16) else wav.float(), lens,
+                                    sample_rate, config.audio_resample_rate)
+            sample["sample_rate"] = config.audio_resample_rate
+            sample["waveform"] = out[None]
+        yield sample
+
+
+def audio_speed_perturb(data: Iterable[dict], config) -> Iterator[dict]:
+    """Speed perturbation.  Same contract and draw as ref: touchnet/data/functions.py:99-114; sox's `speed` + `rate` is
+    done as torchaudio-style sinc resampling from sample_rate*speed to sample_rate (not sox's filter)."""
+    for sample in data:
+        assert "sample_rate" in sample
+        assert "waveform" in sample
+        sample_rate = sample["sample_rate"]
+        speed = random.choice(config.audio_speed_perturb_speeds)
+        if speed != 1.0:
+            wav, lens = _pack([sample["waveform"]], _device(config))
+            out, _ = speed_perturb_batch(wav if wav.dtype in (torch.float32, torch.int16) else wav.float(), lens,
+                                         [speed], sample_rate)
+            sample["waveform"] = out[None]
+        yield sample
+
+
+def audiofeat_spec_aug(data: Iterable[dict], config) -> Iterator[dict]:
+    """SpecAugment time and frequency masks.  Same contract and draws as ref: touchnet/data/functions.py:193-217."""
+    for sample in data:
+        assert "audiofeat" in sample
+        x = sample["audiofeat"]
+        t_masks, f_masks = augment.draw_time_freq_masks(x.size(0), x.size(1), config)
+        yield _apply_feature_ops(sample, config, t_masks=t_masks, f_masks=f_masks)
+
+
+def audiofeat_spec_sub(data: Iterable[dict], config) -> Iterator[dict]:
+    """SpecSub.  Same contract and draws as ref: touchnet/data/functions.py:220-239 (every sub reads the input)."""
+    for sample in data:
+        assert "audiofeat" in sample
+        subs = augment.draw_subs(sample["audiofeat"].size(0), config)
+        yield _apply_feature_ops(sample, config, subs=subs)
+
+
+def audiofeat_spec_trim(data: Iterable[dict], config) -> Iterator[dict]:
+    """SpecTrim (tail frames).  Same contract and draw as ref: touchnet/data/functions.py:242-255."""
+    for sample in data:
+        assert "audiofeat" in sample
+        trim = augment.draw_trim(sample["audiofeat"].size(0), config)
+        yield _apply_feature_ops(sample, config, trim=trim) if trim else sample
