@@ -189,6 +189,17 @@ int tn_greedy_select_bf16(const void* logits, int64_t ld, int B, int V, int64_t*
 int tn_fbank_f32(const void* wav, int wav_is_i16, const int64_t* utt_offsets, const int64_t* frame_offsets, int n_utts,
                  int64_t total_frames, int frame_len, int frame_shift, int n_fft, const float* window,
                  const float* mel_filters, int n_mels, float preemph, float* out, tn_stream_t stream);
+/*   tn_mfcc: touchnet/data/functions.py:137-156 audio_compute_mfcc → ta:compliance/kaldi.py mfcc with the arguments
+ *     the reference leaves at their defaults (use_energy off, cepstral_lifter 22, no htk_compat, no mean subtraction):
+ *     tn_fbank's log-mel row y (same arguments, same arithmetic) times dct [n_mels, n_ceps] fp32, the orthonormal
+ *     DCT-II of torchaudio's _get_dct_matrix with the lifter folded into its columns by the host.  out is
+ *     [total_frames, n_ceps]; the log-mel row never leaves the chip.  c[i] = sum_m y[m] * dct[m][i] in ascending m:
+ *     bit-reproducible.  1 <= n_ceps <= n_mels (the reference asserts the same).
+ */
+int tn_mfcc_f32(const void* wav, int wav_is_i16, const int64_t* utt_offsets, const int64_t* frame_offsets, int n_utts,
+                int64_t total_frames, int frame_len, int frame_shift, int n_fft, const float* window,
+                const float* mel_filters, int n_mels, float preemph, const float* dct /*[n_mels, n_ceps], lifter folded in*/,
+                int n_ceps, float* out, tn_stream_t stream);
 int tn_logmel_power_f32(const float* wav, const int64_t* utt_offsets, const int64_t* frame_offsets, int n_utts,
                         int64_t total_frames, int n_fft, int hop, const float* window, const float* mel_filters,
                         int n_mels, float* out, float* utt_max, tn_stream_t stream);

@@ -5,6 +5,8 @@ GPU (CUDA events, L2 flushed before every timed call, median of --iters):
   plain      fbank_batch + stack_batch(into=...)                         (what bench.py runs)
   augmented  augmented_fbank_stack_batch(into=...) with the recipe's draws: speed {0.9, 1.0, 1.1}, 2 time masks <= 50,
              2 freq masks <= 10, 3 subs <= 30 (examples/audio/sft/asr/wenetspeech/run.sh:258-270), trim off
+  --feat-type mfcc times mfcc_batch / augmented_mfcc_stack_batch instead (80 mel bins, 40 cepstra, frequency masks drawn
+  over the 40 columns) and kaldi.mfcc in the CPU chain.
   and the two augmentation kernels on their own, with achieved algorithmic bytes against the 3.35 TB/s data-sheet HBM3
   bandwidth of the H100 SXM: resample reads each input sample once (2 B int16) and writes each output once (4 B);
   spec augment reads each output frame's source row unless it is zeroed and writes each output frame (4 B * F each).
@@ -65,7 +67,7 @@ def timed(fn, iters, flush):
     return sorted(ts)[len(ts) // 2]
 
 
-def cpu_chain(items):
+def cpu_chain(items, feat_type="fbank"):
     import torchaudio
     from oracle import frontend_oracle as fo
     torch.set_num_threads(1)
@@ -73,8 +75,13 @@ def cpu_chain(items):
         w = torch.from_numpy(pcm.astype(np.float32) / 32768.0)[None]
         if rec["speed"] != 1.0:
             w = torchaudio.transforms.Resample(augment.speed_source_rate(16000, rec["speed"]), 16000)(w)
-        x = torchaudio.compliance.kaldi.fbank(w * 32768, num_mel_bins=80, frame_length=25, frame_shift=10, dither=0.0,
-                                              energy_floor=0.0, sample_frequency=16000)
+        if feat_type == "mfcc":
+            x = torchaudio.compliance.kaldi.mfcc(w * 32768, num_mel_bins=80, frame_length=25, frame_shift=10,
+                                                 dither=0.0, num_ceps=40, high_freq=0.0, low_freq=20.0,
+                                                 sample_frequency=16000)
+        else:
+            x = torchaudio.compliance.kaldi.fbank(w * 32768, num_mel_bins=80, frame_length=25, frame_shift=10,
+                                                  dither=0.0, energy_floor=0.0, sample_frequency=16000)
         y = x.clone()
         for s, e in rec["t_masks"]:
             y[s:e, :] = 0
@@ -93,7 +100,15 @@ def main():
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--seed", type=int, default=0)
     ap.add_argument("--no-cpu", action="store_true")
+    ap.add_argument("--feat-type", choices=("fbank", "mfcc"), default="fbank")
     args = ap.parse_args()
+    mfcc = args.feat_type == "mfcc"
+    if mfcc:
+        CFG.audio_feat_type, CFG.audiofeat_num_ceps = "mfcc", 40
+    n_feat = 40 if mfcc else 80
+    features = ((lambda w, n: frontend.mfcc_batch(w, n, num_mel_bins=80, num_ceps=40)) if mfcc
+                else (lambda w, n: frontend.fbank_batch(w, n)))
+    augmented_stack = frontend.augmented_mfcc_stack_batch if mfcc else frontend.augmented_fbank_stack_batch
     assert torch.cuda.is_available(), "time_augment.py measures on the GPU; there is no CPU fallback"
     dev = torch.device("cuda:0")
     smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
@@ -104,21 +119,21 @@ def main():
     wav, lens = frontend._pack(pcms, dev)
     rows = plan["doc_audio"].tolist()
     dst = plan["doc_off"].tolist()
-    feats = torch.zeros(args.seq_len, 400, device=dev)
+    feats = torch.zeros(args.seq_len, 5 * n_feat, device=dev)
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
     plain_rows = [augment.stacked_rows(frontend.fbank_frames(n, 16000, 25, 10), 4) for n in lens]
     plain_dst = [sum(plain_rows[:i]) for i in range(len(plain_rows))]
-    plain_buf = torch.zeros(sum(plain_rows), 400, device=dev)
+    plain_buf = torch.zeros(sum(plain_rows), 5 * n_feat, device=dev)
 
     def plain():
-        fb, fr = frontend.fbank_batch(wav, lens)
+        fb, fr = features(wav, lens)
         frontend.stack_batch(fb, fr, 5, 4, True, into=plain_buf, dst_rows=plain_dst)
 
     def augmented():
-        frontend.augmented_fbank_stack_batch(wav, lens, recs, into=feats, dst_rows=dst)
+        augmented_stack(wav, lens, recs, into=feats, dst_rows=dst)
 
     sped, slens = frontend.speed_perturb_batch(wav, lens, [r["speed"] for r in recs], 16000)
-    fb, frames = frontend.fbank_batch(sped, slens)
+    fb, frames = features(sped, slens)
     out_frames = [f - r["trim"] for f, r in zip(frames, recs)]
     t_plain = timed(plain, args.iters, flush)
     t_aug = timed(augmented, args.iters, flush)
@@ -127,7 +142,7 @@ def main():
     sa_out, _ = frontend.spec_augment_batch(fb, frames, recs)
     rs_bytes = 2 * sum(lens) + 4 * sum(slens)
     zero_rows = int((sa_out == 0).all(dim=1).sum())
-    sa_bytes = 4 * 80 * (2 * sum(out_frames) - zero_rows)
+    sa_bytes = 4 * n_feat * (2 * sum(out_frames) - zero_rows)
     # kernel-only times from the profiler (the event windows above also hold the host-side table building and copies)
     from torch.profiler import ProfilerActivity, profile
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
@@ -141,13 +156,14 @@ def main():
             if k in e.name and e.device_type == torch.autograd.DeviceType.CUDA:
                 dur[k].append(e.device_time_total / 1e3)
     k_rs, k_sa = (sorted(v)[len(v) // 2] for v in dur.values())
-    res = {"gpu": smi, "utterances": len(lens), "audio_s": sum(lens) / 16000.0, "rows": sum(rows),
+    res = {"gpu": smi, "feat_type": args.feat_type, "utterances": len(lens), "audio_s": sum(lens) / 16000.0, "rows": sum(rows),
            "plain_call_ms": t_plain, "augmented_call_ms": t_aug, "resample_call_ms": t_rs, "spec_augment_call_ms": t_sa,
            "resample_kernel_ms": k_rs, "spec_augment_kernel_ms": k_sa,
            "resample_GBps": rs_bytes / k_rs / 1e6, "resample_pct_hbm": 100 * rs_bytes / k_rs / 1e9 / HBM_TBS,
            "spec_augment_GBps": sa_bytes / k_sa / 1e6, "spec_augment_pct_hbm": 100 * sa_bytes / k_sa / 1e9 / HBM_TBS}
     print(f"GPU: {smi}")
     print(f"one packed row of {args.seq_len}: {len(lens)} utterances, {res['audio_s']:.1f} s of 16 kHz int16 audio")
+    print(f"features: {args.feat_type}")
     print(f"call times (events): plain frontend {t_plain * 1e3:.1f} us, augmented {t_aug * 1e3:.1f} us, "
           f"speed_perturb_batch {t_rs * 1e3:.1f} us, spec_augment_batch {t_sa * 1e3:.1f} us")
     print(f"kernels (profiler): resample {k_rs * 1e3:.1f} us, {res['resample_GBps']:.0f} GB/s = "
@@ -155,12 +171,12 @@ def main():
           f"{res['spec_augment_GBps']:.0f} GB/s = {res['spec_augment_pct_hbm']:.1f} %")
     if not args.no_cpu:
         items = [(p.numpy(), r) for p, r in zip(pcms, recs)]
-        t0 = time.perf_counter(); cpu_chain(items); t1 = time.perf_counter()
+        t0 = time.perf_counter(); cpu_chain(items, args.feat_type); t1 = time.perf_counter()
         n = os.cpu_count() or 1
-        chunks = [items[i::n] for i in range(n)]
+        chunks = [(items[i::n], args.feat_type) for i in range(n)]
         with Pool(n) as pool:
-            pool.map(cpu_chain, [items[:1]] * n)   # warm the workers (imports)
-            t2 = time.perf_counter(); pool.map(cpu_chain, chunks); t3 = time.perf_counter()
+            pool.starmap(cpu_chain, [(items[:1], args.feat_type)] * n)   # warm the workers (imports)
+            t2 = time.perf_counter(); pool.starmap(cpu_chain, chunks); t3 = time.perf_counter()
         res.update(cpu_1thread_ms=(t1 - t0) * 1e3, cpu_procs=n, cpu_procs_ms=(t3 - t2) * 1e3)
         print(f"CPU chain (torchaudio stand-in): 1 thread {res['cpu_1thread_ms']:.0f} ms, "
               f"{n} processes {res['cpu_procs_ms']:.0f} ms")

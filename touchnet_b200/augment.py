@@ -11,7 +11,9 @@ order of touchnet/models/touch_audio/processing_touch_audio.py:453-476):
 
 How many draws a sample consumes, and their ranges, depend only on its length.  So `draw_record` makes them here, in the
 DataLoader worker and in exactly the reference's order, from the waveform length alone; the result is a small record
-that the GPU applies after the H2D copy (`frontend.augmented_fbank_stack_batch`).  No tensor is touched on the host.
+that the GPU applies after the H2D copy (`frontend.augmented_fbank_stack_batch`, or `augmented_mfcc_stack_batch` for
+audio_feat_type "mfcc", whose frames are fbank's and whose frequency masks span the audiofeat_num_ceps columns).  No
+tensor is touched on the host.
 """
 from __future__ import annotations
 
@@ -81,14 +83,19 @@ def sinc_resample_bank(orig: int, new: int, device: str = "cpu") -> tuple[torch.
 # ---------------------------------------------------------------------------------------------------------------
 # feature lengths
 # ---------------------------------------------------------------------------------------------------------------
+def _kaldi_frames(n_samples: int, sample_rate: int, config) -> int:
+    """snip_edges framing of kaldi fbank, which kaldi mfcc shares."""
+    win = int(sample_rate * config.audiofeat_frame_length * 0.001)
+    shift = int(sample_rate * config.audiofeat_frame_shift * 0.001)
+    return 0 if n_samples < win else 1 + (n_samples - win) // shift
+
+
 def feature_frames(n_samples: int, sample_rate: int, config) -> int:
     """Frames the configured feature extractor produces for n_samples (fbank: snip_edges framing; whisper log-mel:
     (n + padding) // hop, ref: functions.py:159-190)."""
     kind = getattr(config, "audio_feat_type", "fbank")
     if kind == "fbank":
-        win = int(sample_rate * config.audiofeat_frame_length * 0.001)
-        shift = int(sample_rate * config.audiofeat_frame_shift * 0.001)
-        return 0 if n_samples < win else 1 + (n_samples - win) // shift
+        return _kaldi_frames(n_samples, sample_rate, config)
     if kind == "log_mel_spectrogram":
         return (n_samples + getattr(config, "audiofeat_padding", 0)) // config.audiofeat_hop_length
     raise TouchNetB200Error(f"augmentation records support audio_feat_type fbank / log_mel_spectrogram, not {kind!r}")
@@ -152,9 +159,12 @@ def draw_record(n_samples: int, sample_rate: int, config, rng=random) -> dict:
         rec["speed"] = float(speed)
         if speed != 1.0:
             n = resampled_length(n, speed_source_rate(sr, speed), sr)
-    frames = feature_frames(n, sr, config)
+    mfcc = getattr(config, "audio_feat_type", "fbank") == "mfcc"
+    frames = _kaldi_frames(n, sr, config) if mfcc else feature_frames(n, sr, config)
     if getattr(config, "audiofeat_spec_aug", False):
-        rec["t_masks"], rec["f_masks"] = draw_time_freq_masks(frames, config.audiofeat_num_mel_bins, config, rng)
+        # frequency masks span the feature's columns (y.size(1) of ref: functions.py:203)
+        n_freq = config.audiofeat_num_ceps if mfcc else config.audiofeat_num_mel_bins
+        rec["t_masks"], rec["f_masks"] = draw_time_freq_masks(frames, n_freq, config, rng)
     if getattr(config, "audiofeat_spec_sub", False):
         rec["subs"] = draw_subs(frames, config, rng)
     if getattr(config, "audiofeat_spec_trim", False):

@@ -1,8 +1,11 @@
-// touchnet_b200 :: audio frontend (waveform -> fbank / log-mel -> stacked low-frame-rate features) on the GPU.
+// touchnet_b200 :: audio frontend (waveform -> fbank / MFCC / log-mel -> stacked low-frame-rate features) on the GPU.
 //
 // Replaces, batched over utterances packed back to back in one buffer:
 //   audio_compute_fbank                touchnet/data/functions.py:117-134
 //       -> torchaudio.compliance.kaldi.fbank  ta:compliance/kaldi.py:514-645 (+ :44-84 framing, :154-217 window)
+//   audio_compute_mfcc                 touchnet/data/functions.py:137-156
+//       -> torchaudio.compliance.kaldi.mfcc   ta:compliance/kaldi.py:679-800: fbank's log-mel row times the DCT table
+//          (the lifter folded in on the host), a compile-time epilogue variant of the two fbank kernels
 //   audio_compute_log_mel_spectrogram  touchnet/data/functions.py:159-190 (whisper-style torch.stft path)
 //   audiofeat_stack                    touchnet/data/functions.py:258-286
 //
@@ -38,9 +41,16 @@ struct FrontendParams {
   const float* window;       // [frame_len]
   const float* mel_filters;  // [n_mels, n_bins]
   float preemph;
-  float* out;      // [total_frames, n_mels]
+  float* out;      // [total_frames, n_mels]  (MFCC: [total_frames, n_ceps])
   float* utt_max;  // whisper mode
+  const float* dct;  // MFCC: [n_mels, n_ceps] DCT-II table with the lifter folded in
+  int n_ceps;
 };
+
+// the MFCC table [n_mels][n_ceps] is staged in shared memory once per CTA (64 KB at the 128 x 128 limit)
+__device__ __forceinline__ void stage_dct(const float* __restrict__ dct, int n_mels, int n_ceps, float* dct_s) {
+  for (int i = threadIdx.x; i < n_mels * n_ceps; i += blockDim.x) dct_s[i] = __ldg(dct + i);
+}
 
 __device__ __forceinline__ void atomic_max_float(float* addr, float v) {
   if (v >= 0.f) atomicMax(reinterpret_cast<int*>(addr), __float_as_int(v));
@@ -77,7 +87,8 @@ __device__ __forceinline__ void mel_spans(const float* __restrict__ filters, int
 
 // MODE 0: kaldi fbank (snip_edges, DC removal, pre-emphasis, window, zero-pad to n_fft, log(max(x, eps)))
 // MODE 1: whisper log-mel (center + reflect padding, window length == n_fft, log10(max(x, 1e-10)), per-utt max)
-template <int MODE>
+// MFCC (MODE 0 only): the log-mel rows stay in shared memory and each output is sum_m y[m] * dct[m][c]
+template <int MODE, bool MFCC = false>
 __global__ void __launch_bounds__(FE_THREADS) frontend_kernel(const FrontendParams p) {
   extern __shared__ float fe_smem[];
   float2* tab = reinterpret_cast<float2*>(fe_smem);                       // [n_fft] (cos, sin)(2*pi*i/n_fft)
@@ -85,6 +96,8 @@ __global__ void __launch_bounds__(FE_THREADS) frontend_kernel(const FrontendPara
   float* ps = xs + FE_MAX_NFFT * FE_FRAMES;                               // [8][FE_MAX_BINS+3] power spectra
   int* mel_lo = reinterpret_cast<int*>(ps + FE_FRAMES * (FE_MAX_BINS + 3));  // [n_mels]
   int* mel_hi = mel_lo + FE_MAX_MELS;
+  float* lm = xs;                                           // MFCC: [8][FE_MAX_MELS] log-mel rows (xs is dead by then)
+  float* dct_s = reinterpret_cast<float*>(mel_hi + FE_MAX_MELS);   // MFCC: [n_mels][n_ceps]
   constexpr int PS_LD = FE_MAX_BINS + 3;
 
   const int tid = threadIdx.x;
@@ -97,6 +110,7 @@ __global__ void __launch_bounds__(FE_THREADS) frontend_kernel(const FrontendPara
     tab[i] = make_float2(c, s);
   }
   mel_spans(p.mel_filters, p.n_mels, n_bins, mel_lo, mel_hi);
+  if constexpr (MFCC) stage_dct(p.dct, p.n_mels, p.n_ceps, dct_s);
   __syncthreads();
 
   const int64_t n_groups = (p.total_frames + FE_FRAMES - 1) / FE_FRAMES;
@@ -202,10 +216,24 @@ __global__ void __launch_bounds__(FE_THREADS) frontend_kernel(const FrontendPara
           const int u = find_utt(p.frame_offsets, p.n_utts, frame);
           atomic_max_float(p.utt_max + u, y);
         }
-        p.out[frame * p.n_mels + m] = y;
+        if constexpr (MFCC) lm[f * FE_MAX_MELS + m] = y;
+        else p.out[frame * p.n_mels + m] = y;
       }
     }
     __syncthreads();
+    if constexpr (MFCC) {
+      // ---------------- stage 4: cepstra, m ascending (fixed order: bit-reproducible) ----------------
+      for (int o = tid; o < FE_FRAMES * p.n_ceps; o += FE_THREADS) {
+        const int f = o / p.n_ceps, c = o - f * p.n_ceps;
+        const int64_t frame = grp * FE_FRAMES + f;
+        if (frame < p.total_frames) {
+          float acc = 0.f;
+          for (int m = 0; m < p.n_mels; ++m) acc = fmaf(lm[f * FE_MAX_MELS + m], dct_s[m * p.n_ceps + c], acc);
+          p.out[frame * p.n_ceps + c] = acc;
+        }
+      }
+      __syncthreads();
+    }
   }
 }
 
@@ -280,6 +308,9 @@ constexpr int FF_MAX_UTT_TAB = 512;   // utterances per launch whose offsets are
 
 __device__ __forceinline__ uint32_t bitrev8(uint32_t x) { return __brev(x) >> 24; }
 
+// MFCC: the log-mel row goes to the warp's (by then dead) FFT buffer instead of HBM, then lane l writes cepstra
+// l, l+32, ..
+template <bool MFCC>
 __global__ void __launch_bounds__(FF_WARPS * 32) fbank_fft_kernel(const FrontendParams p) {
   extern __shared__ float ff_smem[];
   float2* w256 = reinterpret_cast<float2*>(ff_smem);            // [128]  exp(-2*pi*i*k/256)
@@ -293,6 +324,8 @@ __global__ void __launch_bounds__(FF_WARPS * 32) fbank_fft_kernel(const Frontend
   const uint32_t warp = warp_id(), lane = lane_id();
   float2* z = reinterpret_cast<float2*>(reinterpret_cast<float*>(zbase) + warp * PER_WARP);
   float* ps = reinterpret_cast<float*>(z + FF_H);
+  float* lm = reinterpret_cast<float*>(z);                                   // MFCC: [n_mels] log-mel row
+  float* dct_s = reinterpret_cast<float*>(zbase) + FF_WARPS * PER_WARP;      // MFCC: [n_mels][n_ceps]
   const int tid = threadIdx.x;
   for (int i = tid; i < FF_H / 2; i += blockDim.x) {
     float sn, cs;
@@ -309,6 +342,7 @@ __global__ void __launch_bounds__(FF_WARPS * 32) fbank_fft_kernel(const Frontend
   // utterance offset tables in shared memory: the per-frame binary search then never leaves the SM
   const int n_tab = min(p.n_utts + 1, FF_MAX_UTT_TAB);
   for (int i = tid; i < n_tab; i += blockDim.x) { s_frm_off[i] = p.frame_offsets[i]; s_utt_off[i] = p.utt_offsets[i]; }
+  if constexpr (MFCC) stage_dct(p.dct, p.n_mels, p.n_ceps, dct_s);
   __syncthreads();
   const bool tab_ok = p.n_utts + 1 <= FF_MAX_UTT_TAB;
   const int64_t* frm_off = tab_ok ? s_frm_off : p.frame_offsets;
@@ -384,10 +418,46 @@ __global__ void __launch_bounds__(FF_WARPS * 32) fbank_fft_kernel(const Frontend
       const float* wrow = p.mel_filters + int64_t(m) * n_bins;
       float acc = 0.f;
       for (int k = mel_lo[m]; k < mel_hi[m]; ++k) acc = fmaf(ps[k], __ldg(wrow + k), acc);
-      p.out[frame * p.n_mels + m] = logf(fmaxf(acc, 1.1920928955078125e-07f));
+      const float y = logf(fmaxf(acc, 1.1920928955078125e-07f));
+      if constexpr (MFCC) lm[m] = y;
+      else p.out[frame * p.n_mels + m] = y;
+    }
+    if constexpr (MFCC) {
+      // ---- cepstra: c[i] = sum_m y[m] * dct[m][i], m ascending (fixed order: bit-reproducible) ----
+      __syncwarp();
+      constexpr int CPL = FE_MAX_MELS / 32;   // cepstra per lane (n_ceps <= n_mels <= 128)
+      float c[CPL];
+#pragma unroll
+      for (int j = 0; j < CPL; ++j) c[j] = 0.f;
+      for (int m = 0; m < p.n_mels; ++m) {
+        const float y = lm[m];
+        const float* row = dct_s + m * p.n_ceps + lane;
+#pragma unroll
+        for (int j = 0; j < CPL; ++j)
+          if (int(lane) + 32 * j < p.n_ceps) c[j] = fmaf(y, row[32 * j], c[j]);
+      }
+#pragma unroll
+      for (int j = 0; j < CPL; ++j) {
+        const int i = int(lane) + 32 * j;
+        if (i < p.n_ceps) p.out[frame * p.n_ceps + i] = c[j];
+      }
     }
     __syncwarp();
   }
+}
+
+// extra shared memory of the MFCC variants: the DCT table (the log-mel rows reuse buffers that are dead by then)
+static size_t mfcc_smem(const FrontendParams& p) { return sizeof(float) * size_t(p.n_mels) * p.n_ceps; }
+
+// grid of a persistent MFCC launch: as many CTAs as fit at this table size (the grid-stride loops would otherwise
+// run a partial second wave)
+static int mfcc_grid(void (*kernel)(FrontendParams), int threads, size_t smem, int64_t n_groups, int64_t* grid) {
+  TN_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
+  int per_sm = 0;
+  TN_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem));
+  *grid = int64_t(sm_count()) * (per_sm > 0 ? per_sm : 1);
+  if (*grid > n_groups) *grid = n_groups;
+  return TN_OK;
 }
 
 static int launch_fbank_fft(const FrontendParams& p, cudaStream_t stream) {
@@ -396,7 +466,14 @@ static int launch_fbank_fft(const FrontendParams& p, cudaStream_t stream) {
   const int64_t n_groups = (p.total_frames + FF_WARPS - 1) / FF_WARPS;
   int64_t grid = int64_t(sm_count()) * 6;
   if (grid > n_groups) grid = n_groups;
-  fbank_fft_kernel<<<unsigned(grid), FF_WARPS * 32, smem, stream>>>(p);
+  if (p.dct) {
+    const size_t smem_m = smem + mfcc_smem(p);
+    const int rc = mfcc_grid(fbank_fft_kernel<true>, FF_WARPS * 32, smem_m, n_groups, &grid);
+    if (rc != TN_OK) return rc;
+    fbank_fft_kernel<true><<<unsigned(grid), FF_WARPS * 32, smem_m, stream>>>(p);
+  } else {
+    fbank_fft_kernel<false><<<unsigned(grid), FF_WARPS * 32, smem, stream>>>(p);
+  }
   TN_CHECK_CUDA(cudaGetLastError());
   return TN_OK;
 }
@@ -407,8 +484,16 @@ static int launch_frontend(int mode, const FrontendParams& p, cudaStream_t strea
   const int64_t n_groups = (p.total_frames + FE_FRAMES - 1) / FE_FRAMES;
   int64_t grid = int64_t(sm_count()) * 4;
   if (grid > n_groups) grid = n_groups;
-  if (mode == 0) frontend_kernel<0><<<unsigned(grid), FE_THREADS, smem, stream>>>(p);
-  else frontend_kernel<1><<<unsigned(grid), FE_THREADS, smem, stream>>>(p);
+  if (mode == 0 && p.dct) {
+    const size_t smem_m = smem + mfcc_smem(p);
+    const int rc = mfcc_grid(frontend_kernel<0, true>, FE_THREADS, smem_m, n_groups, &grid);
+    if (rc != TN_OK) return rc;
+    frontend_kernel<0, true><<<unsigned(grid), FE_THREADS, smem_m, stream>>>(p);
+  } else if (mode == 0) {
+    frontend_kernel<0><<<unsigned(grid), FE_THREADS, smem, stream>>>(p);
+  } else {
+    frontend_kernel<1><<<unsigned(grid), FE_THREADS, smem, stream>>>(p);
+  }
   TN_CHECK_CUDA(cudaGetLastError());
   return TN_OK;
 }
@@ -417,25 +502,46 @@ static int launch_frontend(int mode, const FrontendParams& p, cudaStream_t strea
 
 using namespace tn;
 
-extern "C" int tn_fbank_f32(const void* wav, int wav_is_i16, const int64_t* utt_offsets, const int64_t* frame_offsets,
-                            int n_utts, int64_t total_frames, int frame_len, int frame_shift, int n_fft,
-                            const float* window, const float* mel_filters, int n_mels, float preemph, float* out,
-                            tn_stream_t stream_) {
-  clear_error();
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  TN_REQUIRE(wav && utt_offsets && frame_offsets && window && mel_filters && out, "tn_fbank_f32: null pointer");
+// fbank (dct == nullptr) or MFCC: shared argument checks and dispatch of tn_fbank_f32 / tn_mfcc_f32
+static int kaldi_features(const char* fn, const void* wav, int wav_is_i16, const int64_t* utt_offsets,
+                          const int64_t* frame_offsets, int n_utts, int64_t total_frames, int frame_len,
+                          int frame_shift, int n_fft, const float* window, const float* mel_filters, int n_mels,
+                          float preemph, const float* dct, int n_ceps, float* out, cudaStream_t stream) {
+  TN_REQUIRE(wav && utt_offsets && frame_offsets && window && mel_filters && out, "%s: null pointer", fn);
   TN_REQUIRE(n_fft <= FE_MAX_NFFT && n_fft % 2 == 0 && frame_len <= n_fft && frame_len >= 2 && frame_shift > 0,
-             "tn_fbank_f32: unsupported geometry frame_len=%d n_fft=%d (max %d)", frame_len, n_fft, FE_MAX_NFFT);
-  TN_REQUIRE(n_mels > 0 && n_mels <= FE_MAX_MELS, "tn_fbank_f32: n_mels=%d out of range (max %d)", n_mels, FE_MAX_MELS);
+             "%s: unsupported geometry frame_len=%d n_fft=%d (max %d)", fn, frame_len, n_fft, FE_MAX_NFFT);
+  TN_REQUIRE(n_mels > 0 && n_mels <= FE_MAX_MELS, "%s: n_mels=%d out of range (max %d)", fn, n_mels, FE_MAX_MELS);
   if (total_frames == 0 || n_utts == 0) return TN_OK;
   FrontendParams p{};
   p.wav = wav; p.wav_is_i16 = wav_is_i16; p.utt_offsets = utt_offsets; p.frame_offsets = frame_offsets;
   p.n_utts = n_utts; p.total_frames = total_frames; p.frame_len = frame_len; p.frame_shift = frame_shift;
   p.n_fft = n_fft; p.n_bins = n_fft / 2 + 1; p.n_mels = n_mels; p.window = window; p.mel_filters = mel_filters;
-  p.preemph = preemph; p.out = out; p.utt_max = nullptr;
+  p.preemph = preemph; p.out = out; p.utt_max = nullptr; p.dct = dct; p.n_ceps = n_ceps;
   static const bool force_dft = getenv("TN_FBANK_DFT") != nullptr;   // A/B switch: table DFT instead of the FFT path
   if (n_fft == FF_N && !force_dft) return launch_fbank_fft(p, stream);
   return launch_frontend(0, p, stream);
+}
+
+extern "C" int tn_fbank_f32(const void* wav, int wav_is_i16, const int64_t* utt_offsets, const int64_t* frame_offsets,
+                            int n_utts, int64_t total_frames, int frame_len, int frame_shift, int n_fft,
+                            const float* window, const float* mel_filters, int n_mels, float preemph, float* out,
+                            tn_stream_t stream_) {
+  clear_error();
+  return kaldi_features("tn_fbank_f32", wav, wav_is_i16, utt_offsets, frame_offsets, n_utts, total_frames, frame_len,
+                        frame_shift, n_fft, window, mel_filters, n_mels, preemph, nullptr, 0, out,
+                        static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int tn_mfcc_f32(const void* wav, int wav_is_i16, const int64_t* utt_offsets, const int64_t* frame_offsets,
+                           int n_utts, int64_t total_frames, int frame_len, int frame_shift, int n_fft,
+                           const float* window, const float* mel_filters, int n_mels, float preemph, const float* dct,
+                           int n_ceps, float* out, tn_stream_t stream_) {
+  clear_error();
+  TN_REQUIRE(dct, "tn_mfcc_f32: null DCT table");
+  TN_REQUIRE(n_ceps >= 1 && n_ceps <= n_mels, "tn_mfcc_f32: n_ceps=%d out of range (1..n_mels=%d)", n_ceps, n_mels);
+  return kaldi_features("tn_mfcc_f32", wav, wav_is_i16, utt_offsets, frame_offsets, n_utts, total_frames, frame_len,
+                        frame_shift, n_fft, window, mel_filters, n_mels, preemph, dct, n_ceps, out,
+                        static_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int tn_logmel_power_f32(const float* wav, const int64_t* utt_offsets, const int64_t* frame_offsets,

@@ -1,10 +1,11 @@
 """GPU audio frontend behind the reference's data-stage interface.
 
 The reference composes per-sample generator stages `f(data: Iterator[dict], config: DataConfig) -> Iterator[dict]`
-(ref: touchnet/data/datapipe.py:183-205).  The three stages on the hot path are mirrored here with the same names,
-argument meaning and dict keys:
+(ref: touchnet/data/datapipe.py:183-205).  The feature stages are mirrored here with the same names, argument meaning
+and dict keys:
 
     audio_compute_fbank                 ref: touchnet/data/functions.py:117-134
+    audio_compute_mfcc                  ref: touchnet/data/functions.py:137-156
     audio_compute_log_mel_spectrogram   ref: touchnet/data/functions.py:159-190
     audiofeat_stack                     ref: touchnet/data/functions.py:258-286
 
@@ -14,12 +15,13 @@ and the recipe's augmentation stages (draws as the reference makes them, applica
     audio_speed_perturb                 ref: touchnet/data/functions.py:99-114
     audiofeat_spec_aug / _sub / _trim   ref: touchnet/data/functions.py:193-255
 
-plus batch-level entry points (`fbank_batch`, `log_mel_batch`, `stack_batch`, `fbank_stack_batch`, `resample_batch`,
-`speed_perturb_batch`, `spec_augment_batch`, `augmented_fbank_stack_batch`) that process a whole packed batch of
+plus batch-level entry points (`fbank_batch`, `mfcc_batch`, `log_mel_batch`, `stack_batch`, `fbank_stack_batch`,
+`resample_batch`, `speed_perturb_batch`, `spec_augment_batch`, `augmented_fbank_stack_batch`,
+`augmented_mfcc_stack_batch`) that process a whole packed batch of
 utterances in one launch each - the form used after the H2D copy in the train step (SURVEY 8(b) "data-frontend
 boundary", option (i)); for augmentation, the records come from augment.draw_stage in the DataLoader worker.  All
-arithmetic happens in libtouchnet_b200.so (csrc/frontend.cu, csrc/augment.cu); windows, mel filter banks and resampling
-banks are small constants built once on the host exactly as the reference's third-party code builds them and cached per
+arithmetic happens in libtouchnet_b200.so (csrc/frontend.cu, csrc/augment.cu); windows, mel filter banks, the MFCC
+DCT table and resampling banks are small constants built once on the host exactly as the reference's third-party code builds them and cached per
 device.
 """
 from __future__ import annotations
@@ -35,6 +37,7 @@ import torch
 from . import _lib, augment
 
 MILLISECONDS_TO_SECONDS = 0.001
+MAX_MEL_BINS = 128        # mel bins the frontend kernels hold on chip (csrc/frontend.cu FE_MAX_MELS)
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -72,6 +75,24 @@ def _kaldi_mel_banks(num_bins: int, n_fft: int, sample_freq: float, low_freq: fl
     down = (right - mel) / (right - center)
     bins = torch.max(torch.zeros(1), torch.min(up, down))
     return torch.nn.functional.pad(bins, (0, 1)).to(torch.float32).contiguous().to(device)
+
+
+@lru_cache(maxsize=None)
+def _kaldi_mfcc_table(n_mels: int, n_ceps: int, lifter: float = 22.0, device: str = "cpu") -> torch.Tensor:
+    """[n_mels, n_ceps] fp32 table A with mfcc = log-mel row @ A.  ta: compliance/kaldi.py _get_dct_matrix
+    (functional.create_dct(n_mels, n_mels, "ortho"), column 0 set to sqrt(1/n_mels), first n_ceps columns) and
+    _get_lifter_coeffs, both with torchaudio's fp32 op sequence; the lifter is folded in as an fp64 product rounded
+    once to fp32."""
+    n = torch.arange(float(n_mels))
+    k = torch.arange(float(n_mels)).unsqueeze(1)
+    dct = torch.cos(math.pi / float(n_mels) * (n + 0.5) * k)
+    dct[0] *= 1.0 / math.sqrt(2.0)
+    dct *= math.sqrt(2.0 / float(n_mels))
+    dct = dct.t()
+    dct[:, 0] = math.sqrt(1 / float(n_mels))
+    dct = dct[:, :n_ceps]
+    lift = 1.0 + 0.5 * lifter * torch.sin(math.pi * torch.arange(n_ceps) / lifter)
+    return (dct.double() * lift.double()).to(torch.float32).contiguous().to(device)
 
 
 @lru_cache(maxsize=None)
@@ -124,13 +145,11 @@ def fbank_frames(n_samples: int, sample_rate: int, frame_length: float, frame_sh
     return 0 if n_samples < win else 1 + (n_samples - win) // shift
 
 
-def fbank_batch(wav: torch.Tensor, lens: Sequence[int], sample_rate: int = 16000, num_mel_bins: int = 80,
-                frame_length: float = 25.0, frame_shift: float = 10.0, low_freq: float = 20.0, high_freq: float = 0.0,
-                preemphasis: float = 0.97):
-    """wav: packed utterances back to back on the GPU, fp32 in [-1,1] or int16 PCM.  Returns (feats [sum m_i, mel]
-    fp32, frame_counts).  Semantics of kaldi.fbank(waveform * 2**15, dither=0, energy_floor=0) per utterance."""
+def _kaldi_batch(name, wav, lens, sample_rate, num_mel_bins, frame_length, frame_shift, low_freq, high_freq,
+                 preemphasis, num_ceps=None):
+    """Framing, window and mel bank shared by fbank_batch (num_ceps None) and mfcc_batch."""
     if not wav.is_cuda:
-        raise _lib.TouchNetB200Error("fbank_batch needs the packed waveform on the GPU (no CPU path)")
+        raise _lib.TouchNetB200Error(f"{name} needs the packed waveform on the GPU (no CPU path)")
     assert wav.dtype in (torch.float32, torch.int16) and wav.dim() == 1
     dev = str(wav.device)
     win = int(sample_rate * frame_length * MILLISECONDS_TO_SECONDS)
@@ -138,16 +157,45 @@ def fbank_batch(wav: torch.Tensor, lens: Sequence[int], sample_rate: int = 16000
     n_fft = 1 << (win - 1).bit_length()
     frames = [0 if n < win else 1 + (n - win) // shift for n in lens]
     total = int(sum(frames))
-    out = torch.empty((total, num_mel_bins), dtype=torch.float32, device=wav.device)
+    out = torch.empty((total, num_mel_bins if num_ceps is None else num_ceps), dtype=torch.float32, device=wav.device)
     if total == 0:
         return out, frames
     utt_off, frm_off = _offsets(lens, wav.device), _offsets(frames, wav.device)
     window = _povey_window(win, dev)
     banks = _kaldi_mel_banks(num_mel_bins, n_fft, float(sample_rate), float(low_freq), float(high_freq), dev)
-    _lib.call("tn_fbank_f32", wav.data_ptr(), int(wav.dtype == torch.int16), utt_off.data_ptr(), frm_off.data_ptr(),
-              len(lens), total, win, shift, n_fft, window.data_ptr(), banks.data_ptr(), num_mel_bins, float(preemphasis),
-              out.data_ptr(), _st())
+    args = (wav.data_ptr(), int(wav.dtype == torch.int16), utt_off.data_ptr(), frm_off.data_ptr(), len(lens), total, win,
+            shift, n_fft, window.data_ptr(), banks.data_ptr(), num_mel_bins, float(preemphasis))
+    if num_ceps is None:
+        _lib.call("tn_fbank_f32", *args, out.data_ptr(), _st())
+    else:
+        table = _kaldi_mfcc_table(num_mel_bins, num_ceps, 22.0, dev)
+        _lib.call("tn_mfcc_f32", *args, table.data_ptr(), num_ceps, out.data_ptr(), _st())
     return out, frames
+
+
+def fbank_batch(wav: torch.Tensor, lens: Sequence[int], sample_rate: int = 16000, num_mel_bins: int = 80,
+                frame_length: float = 25.0, frame_shift: float = 10.0, low_freq: float = 20.0, high_freq: float = 0.0,
+                preemphasis: float = 0.97):
+    """wav: packed utterances back to back on the GPU, fp32 in [-1,1] or int16 PCM.  Returns (feats [sum m_i, mel]
+    fp32, frame_counts).  Semantics of kaldi.fbank(waveform * 2**15, dither=0, energy_floor=0) per utterance."""
+    return _kaldi_batch("fbank_batch", wav, lens, sample_rate, num_mel_bins, frame_length, frame_shift, low_freq,
+                        high_freq, preemphasis)
+
+
+def mfcc_batch(wav: torch.Tensor, lens: Sequence[int], sample_rate: int = 16000, num_mel_bins: int = 80,
+               num_ceps: int = 40, frame_length: float = 25.0, frame_shift: float = 10.0, low_freq: float = 20.0,
+               high_freq: float = 0.0):
+    """MFCC per utterance of a packed batch (fp32 in [-1,1] or int16 PCM, on the GPU), one launch.  Returns
+    (feats [sum m_i, num_ceps] fp32, frame_counts); frames as fbank_batch.  Semantics of
+    kaldi.mfcc(waveform * 2**15, dither=0, num_ceps, low_freq, high_freq) with torchaudio's other defaults (no energy,
+    lifter 22), ref: functions.py:137-156: fbank's log-mel row times the lifted DCT table, fused into the fbank kernel."""
+    if not 1 <= int(num_ceps) <= int(num_mel_bins):
+        raise _lib.TouchNetB200Error(f"mfcc needs 1 <= num_ceps <= num_mel_bins, got num_ceps={num_ceps}, "
+                                     f"num_mel_bins={num_mel_bins}")
+    if int(num_mel_bins) > MAX_MEL_BINS:
+        raise _lib.TouchNetB200Error(f"mfcc takes at most {MAX_MEL_BINS} mel bins, got {num_mel_bins}")
+    return _kaldi_batch("mfcc_batch", wav, lens, sample_rate, num_mel_bins, frame_length, frame_shift, low_freq,
+                        high_freq, 0.97, int(num_ceps))
 
 
 def log_mel_batch(wav: torch.Tensor, lens: Sequence[int], sample_rate: int = 16000, n_fft: int = 400,
@@ -307,13 +355,9 @@ def spec_augment_batch(feats: torch.Tensor, frames: Sequence[int], records: Sequ
     return out, out_frames
 
 
-def augmented_fbank_stack_batch(wav: torch.Tensor, lens: Sequence[int], records: Sequence[dict], *, sample_rate=16000,
-                                num_mel_bins=80, frame_length=25.0, frame_shift=10.0, stack_length=5, stride_length=4,
-                                normalize=True, into: torch.Tensor | None = None, dst_rows: Sequence[int] | None = None):
-    """The recipe's chain resample -> speed perturb -> fbank -> SpecAugment -> SpecSub -> SpecTrim -> stack on a packed
-    batch of raw waveforms (fp32 or int16), applying the host-drawn records of augment.draw_record / draw_stage.
-    sample_rate is the rate features are computed at (the records' resampling target).  Stages no utterance needs are
-    skipped, so with every augmentation off this is exactly fbank_batch + stack_batch.  Returns stack_batch's result."""
+def _augmented_stack(wav, lens, records, sample_rate, features, stack_length, stride_length, normalize, into, dst_rows):
+    """resample -> speed perturb -> features(wav, lens) -> SpecAugment / SpecSub / SpecTrim -> stack, skipping the stages
+    no utterance needs."""
     if len(records) != len(lens):
         raise _lib.TouchNetB200Error(f"{len(lens)} utterances but {len(records)} records")
     for r in records:
@@ -323,10 +367,35 @@ def augmented_fbank_stack_batch(wav: torch.Tensor, lens: Sequence[int], records:
         wav, lens = _resample_pairs(wav, lens, [r["resample"] for r in records])
     if any(float(r["speed"]) != 1.0 for r in records):
         wav, lens = speed_perturb_batch(wav, lens, [r["speed"] for r in records], sample_rate)
-    feats, frames = fbank_batch(wav, lens, sample_rate, num_mel_bins, frame_length, frame_shift)
+    feats, frames = features(wav, lens)
     if any(augment.record_has_feature_ops(r) for r in records):
         feats, frames = spec_augment_batch(feats, frames, records)
     return stack_batch(feats, frames, stack_length, stride_length, normalize, into=into, dst_rows=dst_rows)
+
+
+def augmented_fbank_stack_batch(wav: torch.Tensor, lens: Sequence[int], records: Sequence[dict], *, sample_rate=16000,
+                                num_mel_bins=80, frame_length=25.0, frame_shift=10.0, stack_length=5, stride_length=4,
+                                normalize=True, into: torch.Tensor | None = None, dst_rows: Sequence[int] | None = None):
+    """The recipe's chain resample -> speed perturb -> fbank -> SpecAugment -> SpecSub -> SpecTrim -> stack on a packed
+    batch of raw waveforms (fp32 or int16), applying the host-drawn records of augment.draw_record / draw_stage.
+    sample_rate is the rate features are computed at (the records' resampling target).  Stages no utterance needs are
+    skipped, so with every augmentation off this is exactly fbank_batch + stack_batch.  Returns stack_batch's result."""
+    return _augmented_stack(wav, lens, records, sample_rate,
+                            lambda w, n: fbank_batch(w, n, sample_rate, num_mel_bins, frame_length, frame_shift),
+                            stack_length, stride_length, normalize, into, dst_rows)
+
+
+def augmented_mfcc_stack_batch(wav: torch.Tensor, lens: Sequence[int], records: Sequence[dict], *, sample_rate=16000,
+                               num_mel_bins=80, num_ceps=40, frame_length=25.0, frame_shift=10.0, low_freq=20.0,
+                               high_freq=0.0, stack_length=5, stride_length=4, normalize=True,
+                               into: torch.Tensor | None = None, dst_rows: Sequence[int] | None = None):
+    """augmented_fbank_stack_batch with MFCC features: resample -> speed perturb -> MFCC -> SpecAugment -> SpecSub ->
+    SpecTrim -> stack, for records drawn with audio_feat_type="mfcc" (frequency masks over the num_ceps columns).
+    With every augmentation off this is exactly mfcc_batch + stack_batch.  Returns stack_batch's result."""
+    return _augmented_stack(wav, lens, records, sample_rate,
+                            lambda w, n: mfcc_batch(w, n, sample_rate, num_mel_bins, num_ceps, frame_length,
+                                                    frame_shift, low_freq, high_freq),
+                            stack_length, stride_length, normalize, into, dst_rows)
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -347,6 +416,23 @@ def audio_compute_fbank(data: Iterable[dict], config) -> Iterator[dict]:
                              frame_length=config.audiofeat_frame_length, frame_shift=config.audiofeat_frame_shift)
         if getattr(config, "audiofeat_dither", 0.0) != 0.0:
             raise _lib.TouchNetB200Error("dither != 0 is not supported (all reference recipes use 0.0)")
+        sample["audiofeat"] = mat
+        yield sample
+
+
+def audio_compute_mfcc(data: Iterable[dict], config) -> Iterator[dict]:
+    """Extract MFCC.  Same contract as ref: touchnet/data/functions.py:137-156."""
+    for sample in data:
+        assert "sample_rate" in sample
+        assert "waveform" in sample
+        if getattr(config, "audiofeat_dither", 0.0) != 0.0:
+            raise _lib.TouchNetB200Error("dither != 0 is not supported (all reference recipes use 0.0)")
+        wav, lens = _pack([sample["waveform"]], _device(config))
+        mat, _ = mfcc_batch(wav.float() if wav.dtype not in (torch.float32, torch.int16) else wav, lens,
+                            sample_rate=sample["sample_rate"], num_mel_bins=config.audiofeat_num_mel_bins,
+                            num_ceps=config.audiofeat_num_ceps, frame_length=config.audiofeat_frame_length,
+                            frame_shift=config.audiofeat_frame_shift, low_freq=config.audiofeat_low_freq,
+                            high_freq=config.audiofeat_high_freq)
         sample["audiofeat"] = mat
         yield sample
 
