@@ -200,9 +200,14 @@ int tn_mfcc_f32(const void* wav, int wav_is_i16, const int64_t* utt_offsets, con
                 int64_t total_frames, int frame_len, int frame_shift, int n_fft, const float* window,
                 const float* mel_filters, int n_mels, float preemph, const float* dct /*[n_mels, n_ceps], lifter folded in*/,
                 int n_ceps, float* out, tn_stream_t stream);
-int tn_logmel_power_f32(const float* wav, const int64_t* utt_offsets, const int64_t* frame_offsets, int n_utts,
-                        int64_t total_frames, int n_fft, int hop, const float* window, const float* mel_filters,
-                        int n_mels, float* out, float* utt_max, tn_stream_t stream);
+/*   tn_logmel_power: wav is fp32 in [-1,1] (wav_is_i16 = 0, used as is: functions.py:168 does not scale it) or int16
+ *     PCM (wav_is_i16 = 1, times 2^-15, so the same bits as fp32 pcm / 32768).  Every utterance is right-padded with
+ *     pad >= 0 zero samples (functions.py:169-170 audiofeat_padding) without a copy: frames reflect-index the padded
+ *     length N_i + pad and read 0 at or past N_i.  frame_offsets counts (N_i + pad) / hop rows per utterance.
+ */
+int tn_logmel_power_f32(const void* wav, int wav_is_i16, const int64_t* utt_offsets, const int64_t* frame_offsets,
+                        int n_utts, int64_t total_frames, int n_fft, int hop, int pad, const float* window,
+                        const float* mel_filters, int n_mels, float* out, float* utt_max, tn_stream_t stream);
 int tn_logmel_finish_f32(float* feats, const int64_t* frame_offsets, const float* utt_max, int n_utts,
                          int64_t total_frames, int n_mels, tn_stream_t stream);
 int tn_feat_stack_f32(const float* feats, const int64_t* frame_offsets, const int64_t* out_offsets, int n_utts,

@@ -6,13 +6,15 @@ GPU (CUDA events, L2 flushed before every timed call, median of --iters):
   augmented  augmented_fbank_stack_batch(into=...) with the recipe's draws: speed {0.9, 1.0, 1.1}, 2 time masks <= 50,
              2 freq masks <= 10, 3 subs <= 30 (examples/audio/sft/asr/wenetspeech/run.sh:258-270), trim off
   --feat-type mfcc times mfcc_batch / augmented_mfcc_stack_batch instead (80 mel bins, 40 cepstra, frequency masks drawn
-  over the 40 columns) and kaldi.mfcc in the CPU chain.
+  over the 40 columns) and kaldi.mfcc in the CPU chain; --feat-type log_mel_spectrogram times log_mel_batch /
+  augmented_log_mel_stack_batch (whisper log-mel, n_fft 400, hop 160, 80 mel bins, audiofeat_padding 0) and the
+  reference's torch.stft path in the CPU chain.
   and the two augmentation kernels on their own, with achieved algorithmic bytes against the 3.35 TB/s data-sheet HBM3
   bandwidth of the H100 SXM: resample reads each input sample once (2 B int16) and writes each output once (4 B);
   spec augment reads each output frame's source row unless it is zeroed and writes each output frame (4 B * F each).
 CPU: the same chain with the same stand-in for sox (torchaudio.transforms.Resample from sr*speed to sr), then
-  torchaudio.compliance.kaldi.fbank, the masks / subs as slice copies on a cloned tensor, and the oracle's stack -
-  one process with one thread, and os.cpu_count() single-thread processes.
+  torchaudio.compliance.kaldi.fbank (or the feature type's features), the masks / subs as slice copies on a cloned
+  tensor, and the oracle's stack - one process with one thread, and os.cpu_count() single-thread processes.
 Prints the GPU name, power limit and SM clocks it ran at, then one JSON line."""
 import argparse
 import json
@@ -75,7 +77,12 @@ def cpu_chain(items, feat_type="fbank"):
         w = torch.from_numpy(pcm.astype(np.float32) / 32768.0)[None]
         if rec["speed"] != 1.0:
             w = torchaudio.transforms.Resample(augment.speed_source_rate(16000, rec["speed"]), 16000)(w)
-        if feat_type == "mfcc":
+        if feat_type == "log_mel_spectrogram":      # ref: functions.py:168-189 (padding 0)
+            stft = torch.stft(w[0], 400, 160, window=torch.hann_window(400), return_complex=True)
+            mel = frontend._slaney_mel_filters(16000, 400, 80, "cpu") @ (stft[..., :-1].abs() ** 2)
+            x = torch.clamp(mel, min=1e-10).log10()
+            x = ((torch.maximum(x, x.max() - 8.0) + 4.0) / 4.0).transpose(0, 1)
+        elif feat_type == "mfcc":
             x = torchaudio.compliance.kaldi.mfcc(w * 32768, num_mel_bins=80, frame_length=25, frame_shift=10,
                                                  dither=0.0, num_ceps=40, high_freq=0.0, low_freq=20.0,
                                                  sample_frequency=16000)
@@ -100,15 +107,20 @@ def main():
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--seed", type=int, default=0)
     ap.add_argument("--no-cpu", action="store_true")
-    ap.add_argument("--feat-type", choices=("fbank", "mfcc"), default="fbank")
+    ap.add_argument("--feat-type", choices=("fbank", "mfcc", "log_mel_spectrogram"), default="fbank")
     args = ap.parse_args()
     mfcc = args.feat_type == "mfcc"
+    CFG.audio_feat_type = args.feat_type
     if mfcc:
-        CFG.audio_feat_type, CFG.audiofeat_num_ceps = "mfcc", 40
+        CFG.audiofeat_num_ceps = 40
+    if args.feat_type == "log_mel_spectrogram":
+        CFG.audiofeat_n_fft, CFG.audiofeat_hop_length, CFG.audiofeat_padding = 400, 160, 0
     n_feat = 40 if mfcc else 80
-    features = ((lambda w, n: frontend.mfcc_batch(w, n, num_mel_bins=80, num_ceps=40)) if mfcc
-                else (lambda w, n: frontend.fbank_batch(w, n)))
-    augmented_stack = frontend.augmented_mfcc_stack_batch if mfcc else frontend.augmented_fbank_stack_batch
+    features = {"fbank": lambda w, n: frontend.fbank_batch(w, n),
+                "mfcc": lambda w, n: frontend.mfcc_batch(w, n, num_mel_bins=80, num_ceps=40),
+                "log_mel_spectrogram": lambda w, n: frontend.log_mel_batch(w, n)}[args.feat_type]
+    augmented_stack = {"fbank": frontend.augmented_fbank_stack_batch, "mfcc": frontend.augmented_mfcc_stack_batch,
+                       "log_mel_spectrogram": frontend.augmented_log_mel_stack_batch}[args.feat_type]
     assert torch.cuda.is_available(), "time_augment.py measures on the GPU; there is no CPU fallback"
     dev = torch.device("cuda:0")
     smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
@@ -121,7 +133,7 @@ def main():
     dst = plan["doc_off"].tolist()
     feats = torch.zeros(args.seq_len, 5 * n_feat, device=dev)
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
-    plain_rows = [augment.stacked_rows(frontend.fbank_frames(n, 16000, 25, 10), 4) for n in lens]
+    plain_rows = [augment.stacked_rows(f, 4) for f in features(wav, lens)[1]]
     plain_dst = [sum(plain_rows[:i]) for i in range(len(plain_rows))]
     plain_buf = torch.zeros(sum(plain_rows), 5 * n_feat, device=dev)
 

@@ -1,6 +1,8 @@
-"""Time the GPU fbank kernel, and the MFCC epilogue on the same batch (80 mel / 40 ceps), on a bench-sized batch (CUDA
-events) and report achieved algorithmic GB/s (waveform read once, features written once), with the GPU's name, power
-limit and SM clocks."""
+"""Time the GPU fbank kernel, the MFCC epilogue (80 mel / 40 ceps) and whisper log-mel (80 and 128 mel) on the same
+bench-sized batch (CUDA events) and report achieved algorithmic GB/s (waveform read once, features written once), with
+the GPU's name, power limit and SM clocks.  Log-mel is a 400-point table DFT, so it is also reported as fp32 FLOP/s:
+2 FMAs (re, im) per sample and bin, 2 * 2 * 400 * 201 FLOP per frame, against the 67 TFLOP/s fp32 data-sheet figure of
+the H100 SXM."""
 import os, subprocess, sys, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from touchnet_b200 import frontend
@@ -30,3 +32,8 @@ print(f"fbank {'DFT' if os.environ.get('TN_FBANK_DFT') else 'FFT'}: {sum(frames)
 ms_m, out, frames = timed(lambda: frontend.mfcc_batch(wav, lens, num_mel_bins=80, num_ceps=40))
 alg = wav.numel() * 4 + out.numel() * 4
 print(f"mfcc_batch 80 mel / 40 ceps: {sum(frames)} frames, {ms_m*1e3:.1f} us ({ms_m/ms:.2f}x fbank), algorithmic {alg/1e6:.1f} MB -> {alg/ms_m/1e6:.1f} GB/s, {sum(frames)/ms_m/1e3:.1f} Mframes/s")
+for n_mels in (80, 128):
+    ms_l, out, frames = timed(lambda: frontend.log_mel_batch(wav, lens, num_mel_bins=n_mels))
+    alg = wav.numel() * 4 + out.numel() * 4
+    flop = 4 * 400 * 201 * sum(frames)
+    print(f"log_mel_batch {n_mels} mel: {sum(frames)} frames, {ms_l*1e3:.1f} us ({ms_l/ms:.2f}x fbank), algorithmic {alg/1e6:.1f} MB -> {alg/ms_l/1e6:.1f} GB/s, {sum(frames)/ms_l/1e3:.1f} Mframes/s, DFT {flop/ms_l/1e9:.1f} TFLOP/s = {100*flop/ms_l/1e9/67:.1f} % of 67 TFLOP/s fp32")

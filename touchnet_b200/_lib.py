@@ -46,7 +46,7 @@ _SIGNATURES = {
     "tn_greedy_select_bf16": [_vp, _i64, _i, _i, _vp, _i64, _vp, _vp, _vp, _vp, _f, _i, _i64, _i64, _vp],
     "tn_fbank_f32": [_vp, _i, _vp, _vp, _i, _i64, _i, _i, _i, _vp, _vp, _i, _f, _vp, _vp],
     "tn_mfcc_f32": [_vp, _i, _vp, _vp, _i, _i64, _i, _i, _i, _vp, _vp, _i, _f, _vp, _i, _vp, _vp],
-    "tn_logmel_power_f32": [_vp, _vp, _vp, _i, _i64, _i, _i, _vp, _vp, _i, _vp, _vp, _vp],
+    "tn_logmel_power_f32": [_vp, _i, _vp, _vp, _i, _i64, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp],
     "tn_logmel_finish_f32": [_vp, _vp, _vp, _i, _i64, _i, _vp],
     "tn_feat_stack_f32": [_vp, _vp, _vp, _i, _i64, _i, _i, _i, _i, _vp, _vp, _i64, _vp],
     "tn_resample_f32": [_vp, _i, _vp, _vp, _vp, _vp, _i, _i64, _i, _vp, _i, _vp, _vp, _vp],

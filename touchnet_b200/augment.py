@@ -11,9 +11,10 @@ order of touchnet/models/touch_audio/processing_touch_audio.py:453-476):
 
 How many draws a sample consumes, and their ranges, depend only on its length.  So `draw_record` makes them here, in the
 DataLoader worker and in exactly the reference's order, from the waveform length alone; the result is a small record
-that the GPU applies after the H2D copy (`frontend.augmented_fbank_stack_batch`, or `augmented_mfcc_stack_batch` for
-audio_feat_type "mfcc", whose frames are fbank's and whose frequency masks span the audiofeat_num_ceps columns).  No
-tensor is touched on the host.
+that the GPU applies after the H2D copy (`frontend.augmented_fbank_stack_batch`; `augmented_mfcc_stack_batch` for
+audio_feat_type "mfcc", whose frames are fbank's and whose frequency masks span the audiofeat_num_ceps columns;
+`augmented_log_mel_stack_batch` for "log_mel_spectrogram", whose frames are (n + audiofeat_padding) // hop and whose
+frequency masks span the audiofeat_num_mel_bins columns).  No tensor is touched on the host.
 """
 from __future__ import annotations
 

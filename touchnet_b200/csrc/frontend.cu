@@ -45,6 +45,7 @@ struct FrontendParams {
   float* utt_max;  // whisper mode
   const float* dct;  // MFCC: [n_mels, n_ceps] DCT-II table with the lifter folded in
   int n_ceps;
+  int pad;           // whisper mode: zero samples appended to every utterance (audiofeat_padding)
 };
 
 // the MFCC table [n_mels][n_ceps] is staged in shared memory once per CTA (64 KB at the 128 x 128 limit)
@@ -98,6 +99,7 @@ __global__ void __launch_bounds__(FE_THREADS) frontend_kernel(const FrontendPara
   int* mel_hi = mel_lo + FE_MAX_MELS;
   float* lm = xs;                                           // MFCC: [8][FE_MAX_MELS] log-mel rows (xs is dead by then)
   float* dct_s = reinterpret_cast<float*>(mel_hi + FE_MAX_MELS);   // MFCC: [n_mels][n_ceps]
+  float* fmax_s = reinterpret_cast<float*>(mel_hi + FE_MAX_MELS);  // MODE 1: [8] log-mel max of each frame of the group
   constexpr int PS_LD = FE_MAX_BINS + 3;
 
   const int tid = threadIdx.x;
@@ -111,6 +113,7 @@ __global__ void __launch_bounds__(FE_THREADS) frontend_kernel(const FrontendPara
   }
   mel_spans(p.mel_filters, p.n_mels, n_bins, mel_lo, mel_hi);
   if constexpr (MFCC) stage_dct(p.dct, p.n_mels, p.n_ceps, dct_s);
+  if constexpr (MODE == 1) if (tid < FE_FRAMES) fmax_s[tid] = -INFINITY;
   __syncthreads();
 
   const int64_t n_groups = (p.total_frames + FE_FRAMES - 1) / FE_FRAMES;
@@ -135,17 +138,22 @@ __global__ void __launch_bounds__(FE_THREADS) frontend_kernel(const FrontendPara
         const int j = int(lane) + 32 * i;
         float x = 0.f;
         if (valid && j < p.frame_len) {
-          int64_t idx;
           if (MODE == 0) {
-            idx = fi * p.frame_shift + j;  // snip_edges: every frame fits
+            const int64_t idx = fi * p.frame_shift + j;  // snip_edges: every frame fits
+            if (p.wav_is_i16) x = float(reinterpret_cast<const int16_t*>(p.wav)[wav0 + idx]);
+            else x = reinterpret_cast<const float*>(p.wav)[wav0 + idx] * 32768.f;
           } else {
-            idx = fi * p.frame_shift + j - n_fft / 2;  // center=True, reflect
+            // center=True, reflect on the right-padded length wav_n + pad; indices past wav_n are the zero padding
+            const int64_t len = wav_n + p.pad;
+            int64_t idx = fi * p.frame_shift + j - n_fft / 2;
             if (idx < 0) idx = -idx;
-            if (idx >= wav_n) idx = 2 * (wav_n - 1) - idx;
+            if (idx >= len) idx = 2 * (len - 1) - idx;
             if (idx < 0) idx = 0;
+            if (idx < wav_n) {
+              if (p.wav_is_i16) x = float(reinterpret_cast<const int16_t*>(p.wav)[wav0 + idx]) * (1.f / 32768.f);
+              else x = reinterpret_cast<const float*>(p.wav)[wav0 + idx];
+            }
           }
-          if (p.wav_is_i16) x = float(reinterpret_cast<const int16_t*>(p.wav)[wav0 + idx]);
-          else x = reinterpret_cast<const float*>(p.wav)[wav0 + idx] * (MODE == 0 ? 32768.f : 1.f);
         }
         v[i] = x;
         sum += x;
@@ -213,14 +221,22 @@ __global__ void __launch_bounds__(FE_THREADS) frontend_kernel(const FrontendPara
           y = logf(fmaxf(acc, 1.1920928955078125e-07f));  // torch.finfo(float32).eps
         } else {
           y = log10f(fmaxf(acc, 1e-10f));
-          const int u = find_utt(p.frame_offsets, p.n_utts, frame);
-          atomic_max_float(p.utt_max + u, y);
+          atomic_max_float(fmax_s + f, y);
         }
         if constexpr (MFCC) lm[f * FE_MAX_MELS + m] = y;
         else p.out[frame * p.n_mels + m] = y;
       }
     }
     __syncthreads();
+    if constexpr (MODE == 1) {
+      // one global atomic per frame, not per (frame, mel): a max is exact, so utt_max is the same either way
+      if (tid < FE_FRAMES) {
+        const int64_t frame = grp * FE_FRAMES + tid;
+        if (frame < p.total_frames)
+          atomic_max_float(p.utt_max + find_utt(p.frame_offsets, p.n_utts, frame), fmax_s[tid]);
+        fmax_s[tid] = -INFINITY;   // read and reset by the same thread; the next group's stage 3 is two barriers away
+      }
+    }
     if constexpr (MFCC) {
       // ---------------- stage 4: cepstra, m ascending (fixed order: bit-reproducible) ----------------
       for (int o = tid; o < FE_FRAMES * p.n_ceps; o += FE_THREADS) {
@@ -492,7 +508,7 @@ static int launch_frontend(int mode, const FrontendParams& p, cudaStream_t strea
   } else if (mode == 0) {
     frontend_kernel<0><<<unsigned(grid), FE_THREADS, smem, stream>>>(p);
   } else {
-    frontend_kernel<1><<<unsigned(grid), FE_THREADS, smem, stream>>>(p);
+    frontend_kernel<1><<<unsigned(grid), FE_THREADS, smem + sizeof(float) * FE_FRAMES, stream>>>(p);
   }
   TN_CHECK_CUDA(cudaGetLastError());
   return TN_OK;
@@ -544,25 +560,26 @@ extern "C" int tn_mfcc_f32(const void* wav, int wav_is_i16, const int64_t* utt_o
                         static_cast<cudaStream_t>(stream_));
 }
 
-extern "C" int tn_logmel_power_f32(const float* wav, const int64_t* utt_offsets, const int64_t* frame_offsets,
-                                   int n_utts, int64_t total_frames, int n_fft, int hop, const float* window,
-                                   const float* mel_filters, int n_mels, float* out, float* utt_max,
-                                   tn_stream_t stream_) {
+extern "C" int tn_logmel_power_f32(const void* wav, int wav_is_i16, const int64_t* utt_offsets,
+                                   const int64_t* frame_offsets, int n_utts, int64_t total_frames, int n_fft, int hop,
+                                   int pad, const float* window, const float* mel_filters, int n_mels, float* out,
+                                   float* utt_max, tn_stream_t stream_) {
   clear_error();
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   TN_REQUIRE(wav && utt_offsets && frame_offsets && window && mel_filters && out && utt_max,
              "tn_logmel_power_f32: null pointer");
   TN_REQUIRE(n_fft <= FE_MAX_NFFT && n_fft % 2 == 0 && hop > 0, "tn_logmel_power_f32: unsupported n_fft=%d", n_fft);
   TN_REQUIRE(n_mels > 0 && n_mels <= FE_MAX_MELS, "tn_logmel_power_f32: n_mels=%d out of range", n_mels);
+  TN_REQUIRE(pad >= 0, "tn_logmel_power_f32: negative padding %d", pad);
   if (n_utts == 0) return TN_OK;
   fill_kernel<<<(n_utts + 255) / 256, 256, 0, stream>>>(utt_max, n_utts, -INFINITY);
   TN_CHECK_CUDA(cudaGetLastError());
   if (total_frames == 0) return TN_OK;
   FrontendParams p{};
-  p.wav = wav; p.wav_is_i16 = 0; p.utt_offsets = utt_offsets; p.frame_offsets = frame_offsets;
+  p.wav = wav; p.wav_is_i16 = wav_is_i16; p.utt_offsets = utt_offsets; p.frame_offsets = frame_offsets;
   p.n_utts = n_utts; p.total_frames = total_frames; p.frame_len = n_fft; p.frame_shift = hop;
   p.n_fft = n_fft; p.n_bins = n_fft / 2 + 1; p.n_mels = n_mels; p.window = window; p.mel_filters = mel_filters;
-  p.preemph = 0.f; p.out = out; p.utt_max = utt_max;
+  p.preemph = 0.f; p.out = out; p.utt_max = utt_max; p.pad = pad;
   return launch_frontend(1, p, stream);
 }
 

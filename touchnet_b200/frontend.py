@@ -17,7 +17,7 @@ and the recipe's augmentation stages (draws as the reference makes them, applica
 
 plus batch-level entry points (`fbank_batch`, `mfcc_batch`, `log_mel_batch`, `stack_batch`, `fbank_stack_batch`,
 `resample_batch`, `speed_perturb_batch`, `spec_augment_batch`, `augmented_fbank_stack_batch`,
-`augmented_mfcc_stack_batch`) that process a whole packed batch of
+`augmented_mfcc_stack_batch`, `augmented_log_mel_stack_batch`) that process a whole packed batch of
 utterances in one launch each - the form used after the H2D copy in the train step (SURVEY 8(b) "data-frontend
 boundary", option (i)); for augmentation, the records come from augment.draw_stage in the DataLoader worker.  All
 arithmetic happens in libtouchnet_b200.so (csrc/frontend.cu, csrc/augment.cu); windows, mel filter banks, the MFCC
@@ -199,13 +199,21 @@ def mfcc_batch(wav: torch.Tensor, lens: Sequence[int], sample_rate: int = 16000,
 
 
 def log_mel_batch(wav: torch.Tensor, lens: Sequence[int], sample_rate: int = 16000, n_fft: int = 400,
-                  hop_length: int = 160, num_mel_bins: int = 80):
-    """Whisper-style log-mel per utterance (ref: functions.py:159-190).  Returns (feats [sum N_i//hop, mel], counts)."""
+                  hop_length: int = 160, num_mel_bins: int = 80, padding: int = 0):
+    """Whisper-style log-mel per utterance (ref: functions.py:159-190) of a packed batch on the GPU: fp32 in [-1,1] or
+    int16 PCM (read as pcm / 32768, bit-identical to the fp32 input).  Every utterance is right-padded with `padding`
+    zero samples (audiofeat_padding, functions.py:169-170) inside the kernel, without a copy.  Returns
+    (feats [sum (N_i + padding)//hop, mel], counts)."""
+    if wav.dtype not in (torch.float32, torch.int16) or wav.dim() != 1:
+        raise _lib.TouchNetB200Error(f"log_mel_batch takes a 1-D packed fp32 or int16 waveform, got {wav.dtype} "
+                                     f"of rank {wav.dim()}")
+    if int(padding) < 0:
+        raise _lib.TouchNetB200Error(f"log_mel_batch: padding must be >= 0, got {padding}")
     if not wav.is_cuda:
         raise _lib.TouchNetB200Error("log_mel_batch needs the packed waveform on the GPU (no CPU path)")
-    assert wav.dtype == torch.float32 and wav.dim() == 1
     dev = str(wav.device)
-    frames = [n // hop_length for n in lens]       # 1 + N//hop stft frames, last one dropped (:176)
+    padding = int(padding)
+    frames = [(n + padding) // hop_length for n in lens]   # 1 + (N+pad)//hop stft frames, last one dropped (:176)
     total = int(sum(frames))
     out = torch.empty((total, num_mel_bins), dtype=torch.float32, device=wav.device)
     if total == 0:
@@ -214,8 +222,9 @@ def log_mel_batch(wav: torch.Tensor, lens: Sequence[int], sample_rate: int = 160
     utt_max = torch.empty(len(lens), dtype=torch.float32, device=wav.device)
     window = _hann_window(n_fft, dev)
     filters = _slaney_mel_filters(sample_rate, n_fft, num_mel_bins, dev)
-    _lib.call("tn_logmel_power_f32", wav.data_ptr(), utt_off.data_ptr(), frm_off.data_ptr(), len(lens), total, n_fft,
-              hop_length, window.data_ptr(), filters.data_ptr(), num_mel_bins, out.data_ptr(), utt_max.data_ptr(), _st())
+    _lib.call("tn_logmel_power_f32", wav.data_ptr(), int(wav.dtype == torch.int16), utt_off.data_ptr(),
+              frm_off.data_ptr(), len(lens), total, n_fft, hop_length, padding, window.data_ptr(), filters.data_ptr(),
+              num_mel_bins, out.data_ptr(), utt_max.data_ptr(), _st())
     _lib.call("tn_logmel_finish_f32", out.data_ptr(), frm_off.data_ptr(), utt_max.data_ptr(), len(lens), total,
               num_mel_bins, _st())
     return out, frames
@@ -398,6 +407,31 @@ def augmented_mfcc_stack_batch(wav: torch.Tensor, lens: Sequence[int], records: 
                             stack_length, stride_length, normalize, into, dst_rows)
 
 
+def augmented_log_mel_stack_batch(wav: torch.Tensor, lens: Sequence[int], records: Sequence[dict], *,
+                                  sample_rate=16000, num_mel_bins=80, n_fft=400, hop_length=160, padding=0,
+                                  stack_length=5, stride_length=4, normalize=True, into: torch.Tensor | None = None,
+                                  dst_rows: Sequence[int] | None = None):
+    """augmented_fbank_stack_batch with whisper log-mel features: resample -> speed perturb -> log-mel (audiofeat_padding
+    zeros appended, the per-utterance max-8 clamp and (x+4)/4 included, so masked cells are 0 as in the reference) ->
+    SpecAugment -> SpecSub -> SpecTrim -> stack, for records drawn with audio_feat_type="log_mel_spectrogram".  An
+    utterance whose length after augmentation plus padding is at most n_fft // 2 raises, as the reference's reflect
+    padding does.  With every augmentation off this is exactly log_mel_batch + stack_batch.  Returns stack_batch's
+    result."""
+    if int(padding) < 0:
+        raise _lib.TouchNetB200Error(f"log-mel padding must be >= 0, got {padding}")
+
+    def features(w, n):
+        for i, m in enumerate(n):
+            if int(m) + int(padding) <= n_fft // 2:
+                raise _lib.TouchNetB200Error(
+                    f"utterance {i} has {m} samples (+{padding} padding) at {sample_rate} Hz: log-mel's reflect padding "
+                    f"needs more than n_fft // 2 = {n_fft // 2}")
+        return log_mel_batch(w, n, sample_rate, n_fft, hop_length, num_mel_bins, padding)
+
+    return _augmented_stack(wav, lens, records, sample_rate, features, stack_length, stride_length, normalize, into,
+                            dst_rows)
+
+
 # ---------------------------------------------------------------------------------------------------------------
 # per-sample generator stages (the reference's operator interface)
 # ---------------------------------------------------------------------------------------------------------------
@@ -438,17 +472,18 @@ def audio_compute_mfcc(data: Iterable[dict], config) -> Iterator[dict]:
 
 
 def audio_compute_log_mel_spectrogram(data: Iterable[dict], config) -> Iterator[dict]:
-    """Extract whisper-style log mel spectrogram.  Same contract as ref: touchnet/data/functions.py:159-190."""
+    """Extract whisper-style log mel spectrogram.  Same contract as ref: touchnet/data/functions.py:159-190; an int16
+    waveform is read as pcm / 32768 and audiofeat_padding is applied inside the kernel."""
     for sample in data:
         assert "sample_rate" in sample
         assert "waveform" in sample
         waveform = sample["waveform"].squeeze(0)
         pad = getattr(config, "audiofeat_padding", 0)
-        if pad > 0:
-            waveform = torch.nn.functional.pad(waveform, (0, pad))
         wav, lens = _pack([waveform], _device(config))
-        mat, _ = log_mel_batch(wav.float(), lens, sample_rate=sample["sample_rate"], n_fft=config.audiofeat_n_fft,
-                               hop_length=config.audiofeat_hop_length, num_mel_bins=config.audiofeat_num_mel_bins)
+        mat, _ = log_mel_batch(wav if wav.dtype in (torch.float32, torch.int16) else wav.float(), lens,
+                               sample_rate=sample["sample_rate"], n_fft=config.audiofeat_n_fft,
+                               hop_length=config.audiofeat_hop_length, num_mel_bins=config.audiofeat_num_mel_bins,
+                               padding=pad if pad > 0 else 0)
         sample["audiofeat"] = mat
         yield sample
 
