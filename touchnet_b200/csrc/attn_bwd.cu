@@ -91,56 +91,6 @@ __global__ void __launch_bounds__(256) attn_delta_kernel(const bf16* __restrict_
   }
 }
 
-// 16 rows x 128 columns of one warp's accumulator (rows row_a and row_a + 8 of the output, `nrows` valid) -> bf16, times
-// `mul`; with rope_cos the inverse rotation  dx_lo = g_lo*cos + g_hi*sin,  dx_hi = g_hi*cos - g_lo*sin  is applied
-// (pairs (j, j+64) sit in accumulator tiles j and j+8 of the thread; tables indexed by trow_a / trow_a + 8)
-__device__ __forceinline__ void store_acc_rows(bf16* out, int64_t ld, int row_a, int nrows, const float (&acc)[16][4],
-                                               float mul, const bf16* rope_cos, const bf16* rope_sin, int64_t trow_a) {
-  const int cq = 2 * int(threadIdx.x & 3);
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int row = row_a + 8 * h;
-    if (row >= nrows) continue;
-    bf16* o = out + int64_t(row) * ld;
-    if (rope_cos == nullptr) {
-#pragma unroll
-      for (int j = 0; j < 16; ++j)
-        *reinterpret_cast<uint32_t*>(o + 8 * j + cq) = pack_bf16x2(acc[j][2 * h] * mul, acc[j][2 * h + 1] * mul);
-    } else {
-      const int64_t tr = (trow_a + 8 * h) * 64;
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const int c = 8 * j + cq;
-        const uint32_t cw = *reinterpret_cast<const uint32_t*>(rope_cos + tr + c);
-        const uint32_t sw = *reinterpret_cast<const uint32_t*>(rope_sin + tr + c);
-        float lo[2], hi[2];
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const float gl = acc[j][2 * h + e] * mul, gh = acc[j + 8][2 * h + e] * mul;
-          const float cs = e ? bf16hi(cw) : bf16lo(cw), sn = e ? bf16hi(sw) : bf16lo(sw);
-          lo[e] = fmaf(gl, cs, gh * sn);
-          hi[e] = fmaf(gh, cs, -gl * sn);
-        }
-        *reinterpret_cast<uint32_t*>(o + c) = pack_bf16x2(lo[0], lo[1]);
-        *reinterpret_cast<uint32_t*>(o + c + 64) = pack_bf16x2(hi[0], hi[1]);
-      }
-    }
-  }
-}
-
-__device__ __forceinline__ void zero_rows(bf16* out, int64_t ld, int row0, int nrows, int tid) {
-  for (int i = tid; i < ATT_BLK * 16; i += BWD_THREADS) {
-    const int r = row0 + (i >> 4);
-    if (r < nrows) *reinterpret_cast<uint4*>(out + int64_t(r) * ld + (i & 15) * 8) = make_uint4(0, 0, 0, 0);
-  }
-}
-
-// A fragments of a 16 x 16 block of bf16 P / dS values held as two adjacent n8 accumulator tiles
-__device__ __forceinline__ void acc_to_a(const float (&x0)[4], const float (&x1)[4], uint32_t (&a)[4]) {
-  a[0] = pack_bf16x2(x0[0], x0[1]); a[1] = pack_bf16x2(x0[2], x0[3]);
-  a[2] = pack_bf16x2(x1[0], x1[1]); a[3] = pack_bf16x2(x1[2], x1[3]);
-}
-
 // ---------------------------------------------------------------------------------------------------------------
 // dK / dV
 // ---------------------------------------------------------------------------------------------------------------
@@ -149,12 +99,7 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) attn_dkdv_kernel(const AttnBwd
   const uint32_t sb = smem_u32(smem);
   float* sCol = reinterpret_cast<float*>(smem + DkdvSmem::COL);
   int blk, kvh, b;
-  if (p.order) {
-    const int e = p.order[blockIdx.x / p.KV];
-    kvh = int(blockIdx.x % p.KV); b = e / p.nblk; blk = e % p.nblk;
-  } else {
-    blk = blockIdx.x; kvh = blockIdx.y; b = blockIdx.z;
-  }
+  attn_work_item(p.order, p.KV, p.nblk, blk, kvh, b);
   const AttnMeta meta = p.meta[b * p.nblk + blk];
   const int tid = int(threadIdx.x), warp = tid >> 5, lane = tid & 31;
   const int k0 = blk * ATT_BLK;
@@ -169,25 +114,27 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) attn_dkdv_kernel(const AttnBwd
   const int nsub = lq1 > lq0 ? (lq1 - lq0 + ATT_SUB - 1) / ATT_SUB : 0;
   const int n = G * nsub;
   if (n == 0) {   // no query attends here: dK = dV = 0
-    zero_rows(dVb, p.ld1, k0, p.T, tid);
-    zero_rows(dKb, p.ld2, k0, p.T, tid);
+    zero_rows<BWD_THREADS>(dVb, p.ld1, k0, p.T, tid);
+    zero_rows<BWD_THREADS>(dKb, p.ld2, k0, p.T, tid);
     return;
   }
-  load_tile_async<ATT_BLK, BWD_THREADS>(sb + DkdvSmem::K, p.K + int64_t(b) * p.T * p.ldk + kvh * ATT_HD, p.ldk, k0, p.T, tid);
-  load_tile_async<ATT_BLK, BWD_THREADS>(sb + DkdvSmem::V, p.V + int64_t(b) * p.T * p.ldv + kvh * ATT_HD, p.ldv, k0, p.T, tid);
+  load_tile_async<ATT_BLK, BWD_THREADS>(sb + DkdvSmem::K, p.K + int64_t(b) * p.T * p.ldk + kvh * ATT_HD, p.ldk, k0, 0, p.T,
+                                        tid);
+  load_tile_async<ATT_BLK, BWD_THREADS>(sb + DkdvSmem::V, p.V + int64_t(b) * p.T * p.ldv + kvh * ATT_HD, p.ldv, k0, 0, p.T,
+                                        tid);
   auto load_q = [&](int it, int buf) {
     const int h = kvh * G + it / nsub;
     const int r0 = lq0 + (it % nsub) * ATT_SUB;
     load_tile_async<ATT_SUB, BWD_THREADS>(sb + DkdvSmem::Q + buf * STR_TILE, p.Q + int64_t(b) * p.Tq * p.ldq + h * ATT_HD,
-                                          p.ldq, r0, p.Tq, tid);
+                                          p.ldq, r0, 0, p.Tq, tid);
     load_tile_async<ATT_SUB, BWD_THREADS>(sb + DkdvSmem::DO + buf * STR_TILE, p.dO + int64_t(b) * p.Tq * p.lddo + h * ATT_HD,
-                                          p.lddo, r0, p.Tq, tid);
+                                          p.lddo, r0, 0, p.Tq, tid);
     if (tid < ATT_SUB) {
       const int r = r0 + tid;
       const bool ok = r < p.Tq && qoff + r < p.T;
       const int64_t li = (int64_t(b) * p.H + h) * p.Tq + r;
       float* col = sCol + buf * 3 * ATT_SUB;
-      col[tid] = ok ? p.lse[li] * 1.4426950408889634f : INFINITY;    // +inf -> P = 0
+      col[tid] = ok ? p.lse[li] * LOG2E : INFINITY;    // +inf -> P = 0
       col[ATT_SUB + tid] = ok ? p.delta[li] : 0.f;
       reinterpret_cast<int32_t*>(col)[2 * ATT_SUB + tid] = ok ? docb[qoff + r] : 0;
     }
@@ -217,82 +164,25 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) attn_dkdv_kernel(const AttnBwd
 
     // S^T = K.Q^T (rows = keys, columns = queries)
     float s[8][4];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) s[j][0] = s[j][1] = s[j][2] = s[j][3] = 0.f;
-#pragma unroll
-    for (int kk = 0; kk < 8; ++kk) {
-      uint32_t af[4];
-      ldsm_a(sb + DkdvSmem::K, warp * 16, kk, af);
-#pragma unroll
-      for (int np = 0; np < 4; ++np) {
-        uint32_t bf[4];
-        ldsm_b_nk(sQ, np * 16, kk, bf);
-        mma_bf16_16816(s[2 * np], af, bf[0], bf[1]);
-        mma_bf16_16816(s[2 * np + 1], af, bf[2], bf[3]);
-      }
-    }
+    mma_scores_nk<4>(s, TileRows{sb + DkdvSmem::K, warp * 16}, sQ, 0);
     // P^T = exp2(S^T * scale_log2 - lse2[q]); masked -> 0
     const bool full = meta.canonical && (k0 + ATT_BLK <= gq0) && d_first > 0 && cdoc[ATT_SUB - 1] == d_first;
+    const DocMask<true> mask{p.scale_log2, full, ka, da, db, gq0, cdoc};
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
+    for (int j = 0; j < 8; ++j)
 #pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int c = 8 * j + cq + (e & 1);
-        float x = s[j][e] * p.scale_log2;
-        if (!full) {
-          const int32_t d = cdoc[c];
-          const bool ok = (e < 2) ? (gq0 + c >= ka && d == da && da > 0) : (gq0 + c >= kb8 && d == db && db > 0);
-          x = ok ? x : -INFINITY;
-        }
-        s[j][e] = fast_exp2(x - col[c]);
-      }
-    }
+      for (int e = 0; e < 4; ++e) s[j][e] = fast_exp2(mask(s[j][e], j, e) - col[8 * j + cq + (e & 1)]);
     // dV += P^T.dO
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {
-      uint32_t a[4];
-      acc_to_a(s[2 * kk], s[2 * kk + 1], a);
-#pragma unroll
-      for (int np = 0; np < 8; ++np) {
-        uint32_t bf[4];
-        ldsm_b_kn(sDO, kk * 16, np, bf);
-        mma_bf16_16816(dv[2 * np], a, bf[0], bf[1]);
-        mma_bf16_16816(dv[2 * np + 1], a, bf[2], bf[3]);
-      }
-    }
+    mma_acc_kn(dv, s, sDO, 0);
     // dP^T = V.dO^T, dS^T = P^T * (dP^T - delta[q])
     float dp[8][4];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) dp[j][0] = dp[j][1] = dp[j][2] = dp[j][3] = 0.f;
-#pragma unroll
-    for (int kk = 0; kk < 8; ++kk) {
-      uint32_t af[4];
-      ldsm_a(sb + DkdvSmem::V, warp * 16, kk, af);
-#pragma unroll
-      for (int np = 0; np < 4; ++np) {
-        uint32_t bf[4];
-        ldsm_b_nk(sDO, np * 16, kk, bf);
-        mma_bf16_16816(dp[2 * np], af, bf[0], bf[1]);
-        mma_bf16_16816(dp[2 * np + 1], af, bf[2], bf[3]);
-      }
-    }
+    mma_scores_nk<4>(dp, TileRows{sb + DkdvSmem::V, warp * 16}, sDO, 0);
 #pragma unroll
     for (int j = 0; j < 8; ++j)
 #pragma unroll
       for (int e = 0; e < 4; ++e) dp[j][e] = s[j][e] * (dp[j][e] - col[ATT_SUB + 8 * j + cq + (e & 1)]);
     // dK += dS^T.Q
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {
-      uint32_t a[4];
-      acc_to_a(dp[2 * kk], dp[2 * kk + 1], a);
-#pragma unroll
-      for (int np = 0; np < 8; ++np) {
-        uint32_t bf[4];
-        ldsm_b_kn(sQ, kk * 16, np, bf);
-        mma_bf16_16816(dk[2 * np], a, bf[0], bf[1]);
-        mma_bf16_16816(dk[2 * np + 1], a, bf[2], bf[3]);
-      }
-    }
+    mma_acc_kn(dk, dp, sQ, 0);
     __syncthreads();   // buffer `buf` is refilled by the next iteration's prefetch
   }
   // dV unscaled; dK carries the softmax scale (and the inverse RoPE when requested)
@@ -308,12 +198,7 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) attn_dq_kernel(const AttnBwdPa
   const uint32_t sb = smem_u32(smem);
   int32_t* sDoc = reinterpret_cast<int32_t*>(smem + DqSmem::DOC);
   int qb, h, b;
-  if (p.order) {
-    const int e = p.order[blockIdx.x / p.H];
-    h = int(blockIdx.x % p.H); b = e / p.nblk; qb = e % p.nblk;
-  } else {
-    qb = blockIdx.x; h = blockIdx.y; b = blockIdx.z;
-  }
+  attn_work_item(p.order, p.H, p.nblk, qb, h, b);
   const int gblk = qb + p.q_blk_off;
   const AttnMeta meta = p.meta[b * p.nblk + gblk];
   const int tid = int(threadIdx.x), warp = tid >> 5, lane = tid & 31;
@@ -323,18 +208,20 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) attn_dq_kernel(const AttnBwdPa
   bf16* dQb = p.out1 + int64_t(b) * p.Tq * p.ld1 + h * ATT_HD;
   const int nsub = meta.kv_end > meta.kv_lo ? (meta.kv_end - meta.kv_lo) * (ATT_BLK / ATT_SUB) : 0;
   if (nsub == 0) {
-    zero_rows(dQb, p.ld1, lrow0, p.Tq, tid);
+    zero_rows<BWD_THREADS>(dQb, p.ld1, lrow0, p.Tq, tid);
     return;
   }
   const bf16* Kb = p.K + int64_t(b) * p.T * p.ldk + kvh * ATT_HD;
   const bf16* Vb = p.V + int64_t(b) * p.T * p.ldv + kvh * ATT_HD;
   const int kbase = meta.kv_lo * ATT_BLK;
-  load_tile_async<ATT_BLK, BWD_THREADS>(sb + DqSmem::Q, p.Q + int64_t(b) * p.Tq * p.ldq + h * ATT_HD, p.ldq, lrow0, p.Tq, tid);
-  load_tile_async<ATT_BLK, BWD_THREADS>(sb + DqSmem::DO, p.dO + int64_t(b) * p.Tq * p.lddo + h * ATT_HD, p.lddo, lrow0, p.Tq, tid);
+  load_tile_async<ATT_BLK, BWD_THREADS>(sb + DqSmem::Q, p.Q + int64_t(b) * p.Tq * p.ldq + h * ATT_HD, p.ldq, lrow0, 0, p.Tq,
+                                        tid);
+  load_tile_async<ATT_BLK, BWD_THREADS>(sb + DqSmem::DO, p.dO + int64_t(b) * p.Tq * p.lddo + h * ATT_HD, p.lddo, lrow0, 0,
+                                        p.Tq, tid);
   auto load_kv = [&](int i, int buf) {
     const int k0 = kbase + i * ATT_SUB;
-    load_tile_async<ATT_SUB, BWD_THREADS>(sb + DqSmem::K + buf * STR_TILE, Kb, p.ldk, k0, p.T, tid);
-    load_tile_async<ATT_SUB, BWD_THREADS>(sb + DqSmem::V + buf * STR_TILE, Vb, p.ldv, k0, p.T, tid);
+    load_tile_async<ATT_SUB, BWD_THREADS>(sb + DqSmem::K + buf * STR_TILE, Kb, p.ldk, k0, 0, p.T, tid);
+    load_tile_async<ATT_SUB, BWD_THREADS>(sb + DqSmem::V + buf * STR_TILE, Vb, p.ldv, k0, 0, p.T, tid);
     if (tid < ATT_SUB) sDoc[buf * ATT_SUB + tid] = (k0 + tid < p.T) ? docb[k0 + tid] : 0;
     cp_async_commit();
   };
@@ -347,10 +234,9 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) attn_dq_kernel(const AttnBwdPa
   const int la = lrow0 + ra, lb = la + 8;
   const float* lseb = p.lse + (int64_t(b) * p.H + h) * p.Tq;
   const float* delb = p.delta + (int64_t(b) * p.H + h) * p.Tq;
-  const float l2a = la < p.Tq ? lseb[la] * 1.4426950408889634f : INFINITY;
-  const float l2b = lb < p.Tq ? lseb[lb] * 1.4426950408889634f : INFINITY;
+  const float l2a = la < p.Tq ? lseb[la] * LOG2E : INFINITY;
+  const float l2b = lb < p.Tq ? lseb[lb] * LOG2E : INFINITY;
   const float dla = la < p.Tq ? delb[la] : 0.f, dlb = lb < p.Tq ? delb[lb] : 0.f;
-  const int cq = 2 * (lane & 3);
   float dq[16][4];
 #pragma unroll
   for (int j = 0; j < 16; ++j) dq[j][0] = dq[j][1] = dq[j][2] = dq[j][3] = 0.f;
@@ -365,55 +251,20 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) attn_dq_kernel(const AttnBwdPa
     const int k0 = kbase + i * ATT_SUB;
 
     float s[8][4], dp[8][4];
-#pragma unroll
-    for (int j = 0; j < 8; ++j)
-#pragma unroll
-      for (int e = 0; e < 4; ++e) { s[j][e] = 0.f; dp[j][e] = 0.f; }
-#pragma unroll
-    for (int kk = 0; kk < 8; ++kk) {
-      uint32_t aq[4], ag[4];
-      ldsm_a(sb + DqSmem::Q, warp * 16, kk, aq);
-      ldsm_a(sb + DqSmem::DO, warp * 16, kk, ag);
-#pragma unroll
-      for (int np = 0; np < 4; ++np) {
-        uint32_t bk[4], bv[4];
-        ldsm_b_nk(sK, np * 16, kk, bk);
-        ldsm_b_nk(sV, np * 16, kk, bv);
-        mma_bf16_16816(s[2 * np], aq, bk[0], bk[1]);
-        mma_bf16_16816(s[2 * np + 1], aq, bk[2], bk[3]);
-        mma_bf16_16816(dp[2 * np], ag, bv[0], bv[1]);
-        mma_bf16_16816(dp[2 * np + 1], ag, bv[2], bv[3]);
-      }
-    }
+    mma_scores_nk<4>(s, TileRows{sb + DqSmem::Q, warp * 16}, sK, 0);
+    mma_scores_nk<4>(dp, TileRows{sb + DqSmem::DO, warp * 16}, sV, 0);
     const bool full = meta.canonical && (k0 + ATT_SUB <= q0) && d_last > 0 && dkd[0] == d_last;
+    const DocMask<false> mask{p.scale_log2, full, qa, da, db, k0, dkd};
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
-        float x = s[j][e] * p.scale_log2;
-        if (!full) {
-          const int c = 8 * j + cq + (e & 1);
-          const int32_t d = dkd[c];
-          const bool ok = (e < 2) ? (k0 + c <= qa && d == da && da > 0) : (k0 + c <= qb8 && d == db && db > 0);
-          x = ok ? x : -INFINITY;
-        }
-        const float pr = fast_exp2(x - (e < 2 ? l2a : l2b));
+        const float pr = fast_exp2(mask(s[j][e], j, e) - (e < 2 ? l2a : l2b));
         dp[j][e] = pr * (dp[j][e] - (e < 2 ? dla : dlb));
       }
     }
     // dQ += dS.K
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {
-      uint32_t a[4];
-      acc_to_a(dp[2 * kk], dp[2 * kk + 1], a);
-#pragma unroll
-      for (int np = 0; np < 8; ++np) {
-        uint32_t bf[4];
-        ldsm_b_kn(sK, kk * 16, np, bf);
-        mma_bf16_16816(dq[2 * np], a, bf[0], bf[1]);
-        mma_bf16_16816(dq[2 * np + 1], a, bf[2], bf[3]);
-      }
-    }
+    mma_acc_kn(dq, dp, sK, 0);
     __syncthreads();
   }
   store_acc_rows(dQb, p.ld1, la, p.Tq, dq, p.scale, p.rope_cos, p.rope_sin, int64_t(b) * p.Tq + la);
@@ -437,10 +288,8 @@ extern "C" int tn_attn_bwd_bf16(const void* Q, int64_t ldq, const void* K, int64
   TN_REQUIRE(B > 0 && T > 0 && H > 0 && KV > 0 && H % KV == 0, "tn_attn_bwd_bf16: bad dims");
   TN_REQUIRE(ldq % 8 == 0 && ldk % 8 == 0 && ldv % 8 == 0 && ldo % 8 == 0 && lddo % 8 == 0 && lddq % 8 == 0 &&
                  lddk % 8 == 0 && lddv % 8 == 0, "tn_attn_bwd_bf16: strides must be multiples of 8");
-  const int nblk = (T + ATT_BLK - 1) / ATT_BLK;
-  if (Tq <= 0) { Tq = T; q_blk_off = 0; }
-  TN_REQUIRE(q_blk_off >= 0 && q_blk_off * ATT_BLK + Tq <= nblk * ATT_BLK, "tn_attn_bwd_bf16: query window outside the sequence");
-  const int nqb = (Tq + ATT_BLK - 1) / ATT_BLK;
+  TN_REQUIRE(attn_query_window(T, Tq, q_blk_off), "tn_attn_bwd_bf16: query window outside the sequence");
+  const int nblk = (T + ATT_BLK - 1) / ATT_BLK, nqb = (Tq + ATT_BLK - 1) / ATT_BLK;
 
   {
     const int64_t pairs = int64_t(B) * Tq * H;
@@ -457,21 +306,15 @@ extern "C" int tn_attn_bwd_bf16(const void* Q, int64_t ldq, const void* K, int64
   p.ldq = ldq; p.ldk = ldk; p.ldv = ldv; p.lddo = lddo;
   p.B = B; p.T = T; p.H = H; p.KV = KV; p.nblk = nblk;
   p.Tq = Tq; p.q_blk_off = q_blk_off;
-  p.scale = scale; p.scale_log2 = scale * 1.4426950408889634f;
+  p.scale = scale; p.scale_log2 = scale * LOG2E;
 
-  static bool configured = false;
-  if (!configured) {
-    TN_CHECK_CUDA(cudaFuncSetAttribute(attn_dkdv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DkdvSmem::TOTAL));
-    TN_CHECK_CUDA(cudaFuncSetAttribute(attn_dq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DqSmem::TOTAL));
-    configured = true;
-  }
+  TN_CHECK_CUDA(attn_smem_optin<attn_dkdv_kernel>(DkdvSmem::TOTAL));
+  TN_CHECK_CUDA(attn_smem_optin<attn_dq_kernel>(DqSmem::TOTAL));
   {
     AttnBwdParams pk = p;
     pk.out1 = static_cast<bf16*>(dV); pk.ld1 = lddv; pk.out2 = static_cast<bf16*>(dK); pk.ld2 = lddk;
     pk.rope_cos = static_cast<const bf16*>(rope_cos_k); pk.rope_sin = static_cast<const bf16*>(rope_sin_k);
-    const bool ordered = (Tq == T && q_blk_off == 0);
-    pk.order = ordered ? meta + attn_meta_order_kv_off(B, nblk) : nullptr;
-    const dim3 grid = ordered ? dim3(unsigned(nblk) * KV * B) : dim3(nblk, KV, B);
+    const dim3 grid = attn_grid(T, Tq, q_blk_off, meta + attn_meta_order_kv_off(B, nblk), nblk, KV, B, pk.order);
     attn_dkdv_kernel<<<grid, BWD_THREADS, DkdvSmem::TOTAL, stream>>>(pk);
     TN_CHECK_CUDA(cudaGetLastError());
   }
@@ -479,9 +322,7 @@ extern "C" int tn_attn_bwd_bf16(const void* Q, int64_t ldq, const void* K, int64
     AttnBwdParams pq = p;
     pq.out1 = static_cast<bf16*>(dQ); pq.ld1 = lddq; pq.out2 = nullptr; pq.ld2 = 0;
     pq.rope_cos = static_cast<const bf16*>(rope_cos_q); pq.rope_sin = static_cast<const bf16*>(rope_sin_q);
-    const bool ordered = (Tq == T && q_blk_off == 0);
-    pq.order = ordered ? meta + attn_meta_order_off(B, nblk) : nullptr;
-    const dim3 grid = ordered ? dim3(unsigned(nqb) * H * B) : dim3(nqb, H, B);
+    const dim3 grid = attn_grid(T, Tq, q_blk_off, meta + attn_meta_order_off(B, nblk), nqb, H, B, pq.order);
     attn_dq_kernel<<<grid, BWD_THREADS, DqSmem::TOTAL, stream>>>(pq);
     TN_CHECK_CUDA(cudaGetLastError());
   }

@@ -47,18 +47,6 @@ struct DecodeParams {
   float scale_log2;
 };
 
-// rows [row0, row0 + 64) of K or V into a swizzled tile; rows outside [lo, hi) are zero-filled (the cache beyond the
-// written length may hold anything, and a NaN there times a zero probability would still be NaN)
-__device__ __forceinline__ void load_kv_tile(uint32_t dst, const bf16* base, int64_t ld, int row0, int lo, int hi, int tid) {
-#pragma unroll
-  for (int i = tid; i < ATT_SUB * 16; i += DEC_THREADS) {
-    const int r = i >> 4, ch = i & 15;
-    const bool ok = row0 + r >= lo && row0 + r < hi;
-    const bf16* src = base + (ok ? int64_t(row0 + r) * ld : 0) + ch * 8;
-    cp_async16(dst + tile_off(r, ch), src, ok ? 16u : 0u);
-  }
-}
-
 __global__ void __launch_bounds__(DEC_THREADS, 2) attn_decode_kernel(const DecodeParams p) {
   extern __shared__ __align__(128) uint8_t smem[];
   const uint32_t sb = smem_u32(smem);
@@ -83,12 +71,12 @@ __global__ void __launch_bounds__(DEC_THREADS, 2) attn_decode_kernel(const Decod
   const uint32_t sQ = sb, sK0 = sb + DEC_Q_TILE, sV0 = sK0 + DEC_STAGES * DEC_SUB_TILE;
 
   // the G query heads of this kv head are rows 0..G-1 of a 16-row tile (rows >= G zero)
-  load_tile_async<16, DEC_THREADS>(sQ, p.Q + int64_t(b) * p.ldq + int64_t(kvh) * G * ATT_HD, ATT_HD, 0, G, tid);
+  load_tile_async<16, DEC_THREADS>(sQ, p.Q + int64_t(b) * p.ldq + int64_t(kvh) * G * ATT_HD, ATT_HD, 0, 0, G, tid);
   auto load_stage = [&](int i) {
     if (i < nsub) {
       const int st = i % DEC_STAGES, k0 = kbase + i * ATT_SUB;
-      load_kv_tile(sK0 + st * DEC_SUB_TILE, Kb, p.ld_tok, k0, lo, hi, tid);
-      load_kv_tile(sV0 + st * DEC_SUB_TILE, Vb, p.ld_tok, k0, lo, hi, tid);
+      load_tile_async<ATT_SUB, DEC_THREADS, true>(sK0 + st * DEC_SUB_TILE, Kb, p.ld_tok, k0, lo, hi, tid);
+      load_tile_async<ATT_SUB, DEC_THREADS, true>(sV0 + st * DEC_SUB_TILE, Vb, p.ld_tok, k0, lo, hi, tid);
     }
     cp_async_commit();   // empty groups keep the group count uniform
   };
@@ -115,50 +103,13 @@ __global__ void __launch_bounds__(DEC_THREADS, 2) attn_decode_kernel(const Decod
     const int k0 = kbase + i * ATT_SUB + warp * 16;   // this warp's 16 keys
 
     float s[2][4];
-#pragma unroll
-    for (int j = 0; j < 2; ++j) s[j][0] = s[j][1] = s[j][2] = s[j][3] = 0.f;
-#pragma unroll
-    for (int kk = 0; kk < 8; ++kk) {
-      uint32_t bf[4];
-      ldsm_b_nk(sK, warp * 16, kk, bf);
-      mma_bf16_16816(s[0], qf[kk], bf[0], bf[1]);
-      mma_bf16_16816(s[1], qf[kk], bf[2], bf[3]);
-    }
-    float mx_a = -INFINITY, mx_b = -INFINITY;
-#pragma unroll
-    for (int j = 0; j < 2; ++j) {
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int key = k0 + 8 * j + cq + (e & 1);
-        const float x = (key >= lo && key < hi) ? s[j][e] * p.scale_log2 : -INFINITY;
-        s[j][e] = x;
-        if (e < 2) mx_a = fmaxf(mx_a, x); else mx_b = fmaxf(mx_b, x);
-      }
-    }
-    mx_a = quad_max(mx_a); mx_b = quad_max(mx_b);
-    const float mn_a = fmaxf(m_a, mx_a), mn_b = fmaxf(m_b, mx_b);
-    const float mu_a = mn_a == -INFINITY ? 0.f : mn_a, mu_b = mn_b == -INFINITY ? 0.f : mn_b;
-    const float al_a = fast_exp2(m_a - mu_a), al_b = fast_exp2(m_b - mu_b);
-    m_a = mn_a; m_b = mn_b;
-    l_a *= al_a; l_b *= al_b;
-#pragma unroll
-    for (int j = 0; j < 16; ++j) { o[j][0] *= al_a; o[j][1] *= al_a; o[j][2] *= al_b; o[j][3] *= al_b; }
-#pragma unroll
-    for (int j = 0; j < 2; ++j) {
-      s[j][0] = fast_exp2(s[j][0] - mu_a); s[j][1] = fast_exp2(s[j][1] - mu_a);
-      s[j][2] = fast_exp2(s[j][2] - mu_b); s[j][3] = fast_exp2(s[j][3] - mu_b);
-      l_a += s[j][0] + s[j][1];
-      l_b += s[j][2] + s[j][3];
-    }
-    const uint32_t a[4] = {pack_bf16x2(s[0][0], s[0][1]), pack_bf16x2(s[0][2], s[0][3]),
-                           pack_bf16x2(s[1][0], s[1][1]), pack_bf16x2(s[1][2], s[1][3])};
-#pragma unroll
-    for (int np = 0; np < 8; ++np) {
-      uint32_t bf[4];
-      ldsm_b_kn(sV, warp * 16, np, bf);
-      mma_bf16_16816(o[2 * np], a, bf[0], bf[1]);
-      mma_bf16_16816(o[2 * np + 1], a, bf[2], bf[3]);
-    }
+    mma_scores_nk<1>(s, qf, sK, warp * 16);
+    const auto mask = [&](float x, int j, int e) {
+      const int key = k0 + 8 * j + cq + (e & 1);
+      return (key >= lo && key < hi) ? x * p.scale_log2 : -INFINITY;
+    };
+    softmax_step(s, mask, o, m_a, m_b, l_a, l_b);
+    mma_acc_kn(o, s, sV, warp * 16);
   }
   cp_async_wait<0>();
   __syncthreads();   // the ring is free: reuse it for the cross-warp merge
@@ -225,10 +176,7 @@ __global__ void __launch_bounds__(ATT_HD) attn_decode_merge_kernel(const float* 
   }
   const float inv = L > 0.f ? 1.f / L : 0.f;
   O[int64_t(b) * ldo + int64_t(h) * ATT_HD + c] = __float2bfloat16_rn(acc * inv);
-  if (lse && c == 0) {
-    constexpr float LN2 = 0.6931471805599453f;
-    lse[int64_t(b) * H + h] = L > 0.f ? (M + __log2f(L)) * LN2 : INFINITY;
-  }
+  if (lse && c == 0) lse[int64_t(b) * H + h] = softmax_lse(M, L);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -360,12 +308,8 @@ extern "C" int tn_attn_decode_bf16(const void* Q, int64_t ldq, const void* K, co
   p.part_ml = workspace + int64_t(B) * H * splits * ATT_HD;
   p.H = H; p.KV = KV; p.S_cap = S_cap; p.splits = splits;
   p.chunk = ((S_cap + splits - 1) / splits + ATT_SUB - 1) / ATT_SUB * ATT_SUB;
-  p.scale_log2 = scale * 1.4426950408889634f;
-  static bool configured = false;
-  if (!configured) {
-    TN_CHECK_CUDA(cudaFuncSetAttribute(attn_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DEC_SMEM));
-    configured = true;
-  }
+  p.scale_log2 = scale * LOG2E;
+  TN_CHECK_CUDA(attn_smem_optin<attn_decode_kernel>(DEC_SMEM));
   attn_decode_kernel<<<dim3(splits, KV, B), DEC_THREADS, DEC_SMEM, stream>>>(p);
   TN_CHECK_CUDA(cudaGetLastError());
   attn_decode_merge_kernel<<<dim3(H, B), ATT_HD, 0, stream>>>(p.part_o, p.part_ml, static_cast<bf16*>(O), ldo, lse, H,
