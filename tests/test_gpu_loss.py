@@ -159,3 +159,78 @@ def test_lazy_logits_route_through_loss_and_accuracy_like_real_logits():
     ref = torch.nn.functional.cross_entropy(m.eval()(input_ids=ids, attention_mask=doc, position_ids=pos).logits.float()
                                             .view(-1, cfg.vocab_size), labels.view(-1), ignore_index=-100)
     assert abs(float(pred.loss) - float(ref)) <= 2e-3 * abs(float(ref))
+
+
+def _ce_rows(M, V, seed):
+    """bf16 logits [M, V] on a 16-byte aligned row stride, labels with ignored rows and one row of equal logits (argmax
+    ties), random sentence lengths."""
+    dev = require_cuda()
+    g = torch.Generator(device=dev).manual_seed(seed)
+    ld = (V + 7) // 8 * 8
+    x = (torch.randn(M, ld, device=dev, generator=g) * 2).bfloat16()[:, :V]
+    x[3] = 0.5
+    labels = torch.randint(0, V, (M,), device=dev, generator=g)
+    labels[-M // 5:] = -100
+    labels[:2] = -100
+    sl = torch.randint(1, 50, (M,), device=dev, generator=g)
+    return x, labels, sl
+
+
+def _bits(t):
+    return t.view({torch.bfloat16: torch.int16, torch.float32: torch.int32}.get(t.dtype, t.dtype))
+
+
+@pytest.mark.parametrize("M,V", [(4096, 128256), (1000, 156032), (700, 1003)])
+def test_fused_ce_kernel_is_bit_identical_to_the_two_pass_kernels(M, V):
+    """tn_pack_ce_fused_bf16 = tn_pack_ce_fwd_bf16 then tn_pack_ce_bwd_bf16 at an upstream gradient of 1: the same lse,
+    ce, argmax and logit gradient, bit for bit."""
+    from touchnet_b200 import _lib
+    x, labels, sl = _ce_rows(M, V, M + V)
+    scale = 1.0 / 7
+    st = torch.cuda.current_stream().cuda_stream
+    out = []
+    for fused in (True, False):
+        xi = torch.empty(M, x.stride(0), dtype=x.dtype, device=x.device)[:, :V].copy_(x)
+        lse = torch.empty(M, dtype=torch.float32, device=x.device)
+        ce = torch.empty_like(lse)
+        am = torch.empty(M, dtype=torch.int32, device=x.device)
+        if fused:
+            _lib.call("tn_pack_ce_fused_bf16", xi.data_ptr(), xi.stride(0), labels.data_ptr(), sl.data_ptr(),
+                      lse.data_ptr(), ce.data_ptr(), am.data_ptr(), scale, M, V, st)
+        else:
+            one = torch.ones(1, dtype=torch.float32, device=x.device)
+            _lib.call("tn_pack_ce_fwd_bf16", xi.data_ptr(), xi.stride(0), labels.data_ptr(), lse.data_ptr(),
+                      ce.data_ptr(), am.data_ptr(), M, V, st)
+            _lib.call("tn_pack_ce_bwd_bf16", xi.data_ptr(), xi.stride(0), labels.data_ptr(), sl.data_ptr(),
+                      lse.data_ptr(), one.data_ptr(), scale, M, V, st)
+        out.append((lse, ce, am, xi))
+    assert int(out[0][2][3]) == 0                                   # the equal row: first index wins
+    for name, a, b in zip(("lse", "ce", "argmax", "dlogits"), *out):
+        assert torch.equal(_bits(a), _bits(b)), name
+
+
+@pytest.mark.parametrize("M,bounds", [(600, (0, 40000, 85000, 128256)), (500, (0, 256, 1003)),
+                                      (300, (0, 8, 4096, 9000, 12347))])
+def test_vocab_parallel_bwd_shards_equal_the_full_bwd(M, bounds):
+    """tn_pack_ce_bwd_vp_bf16 on each column slice [v0, v1) of a row (global labels, the full row's lse) writes exactly
+    what tn_pack_ce_bwd_bf16 writes into those columns of the full row; labels in other shards and ignored rows included."""
+    from touchnet_b200 import _lib
+    V = bounds[-1]
+    x, labels, sl = _ce_rows(M, V, M + len(bounds))
+    labels[5], labels[6], labels[7] = bounds[1], bounds[1] - 1, V - 1       # labels on shard edges
+    st = torch.cuda.current_stream().cuda_stream
+    lse = torch.empty(M, dtype=torch.float32, device=x.device)
+    ce = torch.empty_like(lse)
+    _lib.call("tn_pack_ce_fwd_bf16", x.data_ptr(), x.stride(0), labels.data_ptr(), lse.data_ptr(), ce.data_ptr(), None,
+              M, V, st)
+    g = torch.full((1,), 3.0, dtype=torch.float32, device=x.device)
+    full = torch.empty(M, x.stride(0), dtype=x.dtype, device=x.device)[:, :V].copy_(x)
+    _lib.call("tn_pack_ce_bwd_bf16", full.data_ptr(), full.stride(0), labels.data_ptr(), sl.data_ptr(), lse.data_ptr(),
+              g.data_ptr(), 0.2, M, V, st)
+    shards = torch.empty(M, x.stride(0), dtype=x.dtype, device=x.device)[:, :V].copy_(x)
+    for v0, v1 in zip(bounds[:-1], bounds[1:]):
+        xs = shards[:, v0:v1]
+        _lib.call("tn_pack_ce_bwd_vp_bf16", xs.data_ptr(), xs.stride(0), labels.data_ptr(), sl.data_ptr(), lse.data_ptr(),
+                  g.data_ptr(), 0.2, M, v1 - v0, v0, V, st)
+    assert torch.equal(_bits(shards), _bits(full))
+    assert torch.all(full[labels == -100] == 0)

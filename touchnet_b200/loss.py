@@ -31,30 +31,45 @@ from . import _lib
 _LAST_ARGMAX = None
 
 
-def _check_logits(logits: torch.Tensor) -> None:
-    if not logits.is_cuda or logits.dtype != torch.bfloat16:
-        raise _lib.TouchNetB200Error("pack-loss CE needs bf16 CUDA logits (no CPU path)")
-
-
 def _st() -> int:
     return torch.cuda.current_stream().cuda_stream
+
+
+def _pack_ce_fwd(x: torch.Tensor, labels: torch.Tensor):
+    """(lse, ce, argmax) [M] of the bf16 CUDA logits x [M, V] (unit column stride); contiguous int64 labels outside
+    [0, V) are ignored (ce 0)."""
+    if not x.is_cuda or x.dtype != torch.bfloat16:
+        raise _lib.TouchNetB200Error("pack-loss CE needs bf16 CUDA logits (no CPU path)")
+    assert x.stride(1) == 1
+    M, V = x.shape
+    lse = torch.empty(M, dtype=torch.float32, device=x.device)
+    ce = torch.empty_like(lse)
+    am = torch.empty(M, dtype=torch.int32, device=x.device)
+    _lib.call("tn_pack_ce_fwd_bf16", x.data_ptr(), x.stride(0), labels.data_ptr(), lse.data_ptr(), ce.data_ptr(),
+              am.data_ptr(), M, V, _st())
+    return lse, ce, am
+
+
+def _pack_ce_bwd_(ctx, g_loss, *vp):
+    """Backward of _PackCEFn / _VocabParallelCEFn: overwrites ctx.logits in place with dlogits and returns them in the
+    forward's shape.  vp = (v0, v_total) selects the vocabulary-parallel kernel."""
+    lab, sl, lse = ctx.saved_tensors
+    x = ctx.logits
+    g = g_loss.reshape(1).float().contiguous()
+    _lib.call("tn_pack_ce_bwd_vp_bf16" if vp else "tn_pack_ce_bwd_bf16", x.data_ptr(), x.stride(0), lab.data_ptr(),
+              sl.data_ptr(), lse.data_ptr(), g.data_ptr(), float(ctx.inv_ns), x.shape[0], x.shape[1], *vp, _st())
+    torch.autograd.graph.increment_version(x)   # the kernel overwrote the caller's logits with their gradient: make
+    ctx.logits = None                           # autograd (and accuracy()'s cache key) see the mutation
+    return x.view(ctx.shape)
 
 
 class _PackCEFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, logits, labels, sentence_lens, inv_num_sentence):
-        _check_logits(logits)
-        V = logits.shape[-1]
-        x = logits.view(-1, V)
-        assert x.stride(1) == 1
-        M = x.shape[0]
+        x = logits.view(-1, logits.shape[-1])
         lab = labels.reshape(-1).contiguous()
         sl = sentence_lens.reshape(-1).contiguous()
-        lse = torch.empty(M, dtype=torch.float32, device=x.device)
-        ce = torch.empty(M, dtype=torch.float32, device=x.device)
-        am = torch.empty(M, dtype=torch.int32, device=x.device)
-        _lib.call("tn_pack_ce_fwd_bf16", x.data_ptr(), x.stride(0), lab.data_ptr(), lse.data_ptr(), ce.data_ptr(),
-                  am.data_ptr(), M, V, _st())
+        lse, ce, am = _pack_ce_fwd(x, lab)
         ctx.save_for_backward(lab, sl, lse)
         ctx.logits = x                      # NOT save_for_backward: backward overwrites it in place on purpose
         ctx.inv_ns = inv_num_sentence
@@ -65,14 +80,7 @@ class _PackCEFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g_loss, _g_ce, _g_am):
-        lab, sl, lse = ctx.saved_tensors
-        x = ctx.logits
-        g = g_loss.reshape(1).float().contiguous()
-        _lib.call("tn_pack_ce_bwd_bf16", x.data_ptr(), x.stride(0), lab.data_ptr(), sl.data_ptr(), lse.data_ptr(),
-                  g.data_ptr(), float(ctx.inv_ns), x.shape[0], x.shape[1], _st())
-        torch.autograd.graph.increment_version(x)   # the kernel overwrote the caller's logits with their gradient: make
-        ctx.logits = None                           # autograd (and accuracy()'s cache key) see the mutation
-        return x.view(ctx.shape), None, None, None
+        return _pack_ce_bwd_(ctx, g_loss), None, None, None
 
 
 FUSED_CE_CHUNK = 4096     # token rows per chunk: the [chunk, V] buffer is 1 GB at V = 128 k instead of 2.1 GB for T = 8192;
@@ -134,19 +142,12 @@ class _VocabParallelCEFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, local, labels, sentence_lens, inv_num_sentence, group, v0, v_total):
         import torch.distributed as dist
-        _check_logits(local)
         Vl = local.shape[-1]
         x = local.view(-1, Vl)
-        assert x.stride(1) == 1
-        M = x.shape[0]
         lab = labels.reshape(-1).contiguous()
         sl = sentence_lens.reshape(-1).contiguous()
         lab_l = lab - v0                                                  # out of [0, Vl): "ignored" by the local kernel
-        lse_l = torch.empty(M, dtype=torch.float32, device=x.device)
-        ce_l = torch.empty(M, dtype=torch.float32, device=x.device)
-        am_l = torch.empty(M, dtype=torch.int32, device=x.device)
-        _lib.call("tn_pack_ce_fwd_bf16", x.data_ptr(), x.stride(0), lab_l.data_ptr(), lse_l.data_ptr(), ce_l.data_ptr(),
-                  am_l.data_ptr(), M, Vl, _st())
+        lse_l, ce_l, am_l = _pack_ce_fwd(x, lab_l)
         mine = (lab_l >= 0) & (lab_l < Vl)
         m = lse_l.clone()
         dist.all_reduce(m, op=dist.ReduceOp.MAX, group=group)
@@ -174,14 +175,7 @@ class _VocabParallelCEFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g_loss, _g_ce, _g_am):
-        lab, sl, lse = ctx.saved_tensors
-        x = ctx.logits
-        g = g_loss.reshape(1).float().contiguous()
-        _lib.call("tn_pack_ce_bwd_vp_bf16", x.data_ptr(), x.stride(0), lab.data_ptr(), sl.data_ptr(), lse.data_ptr(),
-                  g.data_ptr(), float(ctx.inv_ns), x.shape[0], x.shape[1], ctx.v0, ctx.v_total, _st())
-        torch.autograd.graph.increment_version(x)
-        ctx.logits = None
-        return x.view(ctx.shape), None, None, None, None, None, None
+        return _pack_ce_bwd_(ctx, g_loss, ctx.v0, ctx.v_total), None, None, None, None, None, None
 
 
 class FusedLinearCEFn(torch.autograd.Function):
@@ -253,22 +247,30 @@ def fused_linear_cross_entropy(hidden: torch.Tensor, weight: torch.Tensor, label
                                  chunk or FUSED_CE_CHUNK)
 
 
+def _handle_loss(pred, labels, sentence_lens, inv_num_sentence: float, detach: bool = False):
+    """(loss_per_sample, ce, argmax) of a LazyLogits / VocabParallelLogits handle; keeps (ce, argmax) on it for accuracy().
+    detach: statistics only, on detached inputs (the fused pass then computes neither dh nor dW)."""
+    if isinstance(pred, LazyLogits):
+        h, w = (pred.hidden.detach(), pred.weight.detach()) if detach else (pred.hidden, pred.weight)
+        out = fused_linear_cross_entropy(h, w, labels, sentence_lens, inv_num_sentence)
+    else:
+        local = pred.local.detach() if detach else pred.local
+        out = _VocabParallelCEFn.apply(local, labels, sentence_lens, inv_num_sentence, pred.group, pred.v0, pred.v_total)
+    pred._stats = out[1:]
+    return out
+
+
 def cross_entropy_loss(pred, labels: torch.Tensor, sentence_lens: torch.Tensor, num_sentence: int,
                        ignore_index: int = -100):
     """Same contract as ref: touchnet/loss/cross_entropy.py:12-50.  Returns (loss_per_sample, loss_per_token).
     `pred` is the model's `pred.logits`: a bf16 [B,T,V] tensor, or a LazyLogits handle (fused lm_head + loss)."""
     assert ignore_index < 0, "labels outside [0, V) are ignored (the reference uses -100)"
     global _LAST_ARGMAX
-    if isinstance(pred, LazyLogits):
-        loss_per_sample, ce, am = fused_linear_cross_entropy(pred.hidden, pred.weight, labels, sentence_lens,
-                                                             1.0 / max(int(num_sentence), 1))
-        pred._stats = (ce, am)
-    elif isinstance(pred, VocabParallelLogits):
-        loss_per_sample, ce, am = _VocabParallelCEFn.apply(pred.local, labels, sentence_lens,
-                                                           1.0 / max(int(num_sentence), 1), pred.group, pred.v0, pred.v_total)
-        pred._stats = (ce, am)
+    inv_num_sentence = 1.0 / max(int(num_sentence), 1)
+    if isinstance(pred, (LazyLogits, VocabParallelLogits)):
+        loss_per_sample, ce, am = _handle_loss(pred, labels, sentence_lens, inv_num_sentence)
     else:
-        loss_per_sample, ce, am = _PackCEFn.apply(pred, labels, sentence_lens, 1.0 / max(int(num_sentence), 1))
+        loss_per_sample, ce, am = _PackCEFn.apply(pred, labels, sentence_lens, inv_num_sentence)
         _LAST_ARGMAX = (weakref.ref(pred), pred._version, am)
     with torch.no_grad():
         num_tokens = (labels != ignore_index).sum()
@@ -277,48 +279,26 @@ def cross_entropy_loss(pred, labels: torch.Tensor, sentence_lens: torch.Tensor, 
     return loss_per_sample, loss_per_token
 
 
-def accuracy(pred: torch.Tensor, labels: torch.Tensor, ignore_index: int = -100) -> torch.Tensor:
-    """Same contract as ref: touchnet/utils/metrics.py:26-50; reuses the argmax the loss kernel already produced."""
-    V = pred.shape[-1]
-    if isinstance(pred, VocabParallelLogits):
-        if pred._stats is None:
-            with torch.no_grad():
-                ones = torch.ones(labels.numel(), dtype=torch.int64, device=labels.device)
-                _, ce, am = _VocabParallelCEFn.apply(pred.local.detach(), labels, ones, 1.0, pred.group, pred.v0, pred.v_total)
-            pred._stats = (ce, am)
-        am = pred._stats[1]
-        lab = labels.reshape(-1)
-        mask = lab != ignore_index
-        num = ((am.long() == lab) & mask).sum()
-        den = mask.sum()
-        return torch.where(den > 0, num / den.clamp(min=1), torch.zeros_like(num, dtype=torch.float32)).detach()
-    if isinstance(pred, LazyLogits):
-        if pred._stats is None:        # accuracy asked before / without the loss: one statistics-only fused pass
-            with torch.no_grad():
-                ones = torch.ones(labels.numel(), dtype=torch.int64, device=labels.device)
-                _, ce, am = fused_linear_cross_entropy(pred.hidden.detach(), pred.weight.detach(), labels, ones, 1.0)
-            pred._stats = (ce, am)
-        am = pred._stats[1]
-        lab = labels.reshape(-1)
-        mask = lab != ignore_index
-        num = ((am.long() == lab) & mask).sum()
-        den = mask.sum()
-        return torch.where(den > 0, num / den.clamp(min=1), torch.zeros_like(num, dtype=torch.float32)).detach()
-    x = pred.view(-1, V)
-    ent = _LAST_ARGMAX
-    if ent is not None and ent[0]() is pred and ent[1] == pred._version and ent[2].numel() == x.shape[0]:
-        am = ent[2]
-    else:
-        _check_logits(pred)
-        M = x.shape[0]
-        lse = torch.empty(M, dtype=torch.float32, device=x.device)
-        ce = torch.empty_like(lse)
-        am = torch.empty(M, dtype=torch.int32, device=x.device)
-        lab = labels.reshape(-1).contiguous()
-        _lib.call("tn_pack_ce_fwd_bf16", x.data_ptr(), x.stride(0), lab.data_ptr(), lse.data_ptr(), ce.data_ptr(),
-                  am.data_ptr(), M, V, _st())
+def _masked_accuracy(am: torch.Tensor, labels: torch.Tensor, ignore_index: int) -> torch.Tensor:
     lab = labels.reshape(-1)
     mask = lab != ignore_index
     num = ((am.long() == lab) & mask).sum()
     den = mask.sum()
     return torch.where(den > 0, num / den.clamp(min=1), torch.zeros_like(num, dtype=torch.float32)).detach()
+
+
+def accuracy(pred: torch.Tensor, labels: torch.Tensor, ignore_index: int = -100) -> torch.Tensor:
+    """Same contract as ref: touchnet/utils/metrics.py:26-50; reuses the argmax the loss kernel already produced."""
+    if isinstance(pred, (LazyLogits, VocabParallelLogits)):
+        if pred._stats is None:        # accuracy asked before / without the loss: one statistics-only pass
+            with torch.no_grad():
+                ones = torch.ones(labels.numel(), dtype=torch.int64, device=labels.device)
+                _handle_loss(pred, labels, ones, 1.0, detach=True)
+        return _masked_accuracy(pred._stats[1], labels, ignore_index)
+    x = pred.view(-1, pred.shape[-1])
+    ent = _LAST_ARGMAX
+    if ent is not None and ent[0]() is pred and ent[1] == pred._version and ent[2].numel() == x.shape[0]:
+        am = ent[2]
+    else:
+        am = _pack_ce_fwd(x, labels.reshape(-1).contiguous())[2]
+    return _masked_accuracy(am, labels, ignore_index)
