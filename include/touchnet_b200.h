@@ -168,6 +168,34 @@ int tn_greedy_select_bf16(const void* logits, int64_t ld, int B, int V, int64_t*
                           float repetition_penalty, int no_repeat_ngram_size, int64_t eos, int64_t pad,
                           tn_stream_t stream);
 
+/* Continuous batching (generation.generate_many): a cache of B slots whose rows are refilled with new prompts while
+ * the other slots keep decoding.  `docs` is a HOST table [n_docs][4] int32 = (src_row, slot, len, limit), at most
+ * TN_ADMIT_MAX documents per call, distinct slots in [0, B), 0 < len < limit <= S_cap; it is checked here and passed to
+ * the kernel by value (no device copy, nothing allocated).
+ *   tn_kv_scatter: cache rows [0, len) of slot `slot` <- source rows [src_row, src_row + len) of K / V (the packed prefill
+ *     of the admitted prompts; n_src_rows rows, strides and alignment as tn_kv_append).  A bit-exact copy; nothing else
+ *     in the cache is written.
+ *   tn_slot_admit: for each document, history[slot, 0:len) = ids[src_row:src_row+len), kv_start[slot] = first row of
+ *     the prompt's last document (its last run of equal doc_ids), kv_end[slot] = len, positions[slot] =
+ *     position_ids[src_row + len - 1], finished[slot] = 0, limit[slot] = limit.  Slots not named are not touched.
+ *   tn_greedy_select_slots: the selection of tn_greedy_select on n_rows logits rows; row r selects for slot
+ *     row_slot[r] (HOST array, at most TN_SELECT_MAX_MAP rows, distinct slots) or, with row_slot = NULL and n_rows == B,
+ *     for slot r.  A slot with finished != 0 (finished or idle) does not advance: next_ids = pad, no history write,
+ *     length and positions unchanged.  A slot finishes when it emits eos or when length + 1 == limit[slot].
+ */
+#define TN_ADMIT_MAX 128
+#define TN_SELECT_MAX_MAP 256
+int tn_kv_scatter_bf16(const void* K, int64_t ldk, const void* V, int64_t ldv, int64_t n_src_rows, void* K_cache,
+                       void* V_cache, int64_t ld_tok, int64_t ld_batch, const int32_t* docs, int n_docs, int B, int S_cap,
+                       int width, tn_stream_t stream);
+int tn_slot_admit(const int32_t* docs, int n_docs, const int64_t* ids, const int32_t* doc_ids, const int64_t* position_ids,
+                  int64_t n_src_rows, int64_t* history, int64_t ld_hist, int32_t* kv_start, int32_t* kv_end,
+                  int64_t* positions, int32_t* finished, int32_t* limit, int B, tn_stream_t stream);
+int tn_greedy_select_slots_bf16(const void* logits, int64_t ld, int n_rows, const int32_t* row_slot, int B, int V,
+                                int64_t* history, int64_t ld_hist, int32_t* length, int64_t* positions, int64_t* next_ids,
+                                int32_t* finished, const int32_t* limit, float repetition_penalty,
+                                int no_repeat_ngram_size, int64_t eos, int64_t pad, tn_stream_t stream);
+
 /* ---------------------------------------------------------------------------------------------------------------
  * Audio frontend.
  *   tn_fbank: touchnet/data/functions.py:117-134 audio_compute_fbank → ta:compliance/kaldi.py:514-645 (snip_edges,

@@ -44,6 +44,10 @@ _SIGNATURES = {
     "tn_attn_decode_bf16": [_vp, _i64, _vp, _vp, _i64, _i64, _vp, _vp, _i, _i, _i, _i, _f, _vp, _vp, _i64, _vp, _vp],
     "tn_kv_append_bf16": [_vp, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _vp, _i, _i, _i, _i, _vp],
     "tn_greedy_select_bf16": [_vp, _i64, _i, _i, _vp, _i64, _vp, _vp, _vp, _vp, _f, _i, _i64, _i64, _vp],
+    "tn_greedy_select_slots_bf16": [_vp, _i64, _i, _vp, _i, _i, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _f, _i, _i64, _i64,
+                                    _vp],
+    "tn_kv_scatter_bf16": [_vp, _i64, _vp, _i64, _i64, _vp, _vp, _i64, _i64, _vp, _i, _i, _i, _i, _vp],
+    "tn_slot_admit": [_vp, _i, _vp, _vp, _vp, _i64, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _i, _vp],
     "tn_fbank_f32": [_vp, _i, _vp, _vp, _i, _i64, _i, _i, _i, _vp, _vp, _i, _f, _vp, _vp],
     "tn_mfcc_f32": [_vp, _i, _vp, _vp, _i, _i64, _i, _i, _i, _vp, _vp, _i, _f, _vp, _i, _vp, _vp],
     "tn_logmel_power_f32": [_vp, _i, _vp, _vp, _i, _i64, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp],

@@ -10,6 +10,10 @@
 // m16n8k16 tile (GQA ratios 1..16), 4 warps each take 16 keys of every 64-key sub-block, K/V sub-blocks arrive through a
 // DEC_STAGES-deep cp.async ring.  Every split writes an fp32 partial (O unnormalised, m in the log2 domain, l); a second
 // kernel merges the splits in split order (no atomics: bit-reproducible run to run).
+//
+// Continuous batching (generation.generate_many) adds slot-addressed forms: a K/V scatter of a packed multi-prompt
+// prefill into chosen cache slots, the admission of those slots' decoding state, and a selection that holds finished /
+// idle slots still and stops a slot at its token limit.
 #include "../../include/touchnet_b200.h"
 #include "attn_common.cuh"
 #include "host.h"
@@ -211,14 +215,24 @@ __device__ __forceinline__ bool argmax_better(float x, int i, float best, int bi
   return i < bi;
 }
 
-__global__ void __launch_bounds__(SEL_THREADS) greedy_select_kernel(
+// The body of both selection kernels.  Logits row r selects for slot b (r == b without a slot map).  SLOTS = false is
+// tn_greedy_select_bf16: every row advances, finished rows take pad.  SLOTS = true is tn_greedy_select_slots_bf16: a
+// finished (or idle) slot does not advance at all (pad in next_ids, nothing else written), and a slot also finishes
+// when its length reaches limit[b].
+template <bool SLOTS>
+__device__ __forceinline__ void greedy_select_row(
     const bf16* __restrict__ logits, int64_t ld, int V, int64_t* __restrict__ history, int64_t ld_hist,
     int32_t* __restrict__ length, int64_t* __restrict__ positions, int64_t* __restrict__ next_ids,
-    int32_t* __restrict__ finished, float penalty, int ngram, int64_t eos, int64_t pad) {
+    int32_t* __restrict__ finished, const int32_t* __restrict__ limit, float penalty, int ngram, int64_t eos,
+    int64_t pad, const int r, const int b) {
   extern __shared__ uint32_t bits[];   // [2][words]: repetition set, banned set
   __shared__ float s_val[SEL_THREADS / 32];
   __shared__ int s_idx[SEL_THREADS / 32];
-  const int b = blockIdx.x, tid = threadIdx.x;
+  const int tid = threadIdx.x;
+  if (SLOTS && finished[b]) {          // uniform over the CTA: no barrier has been reached yet
+    if (tid == 0) next_ids[b] = pad;
+    return;
+  }
   const int words = (V + 31) / 32;
   uint32_t* rep = bits;
   uint32_t* ban = bits + words;
@@ -243,7 +257,7 @@ __global__ void __launch_bounds__(SEL_THREADS) greedy_select_kernel(
     }
   }
   __syncthreads();
-  const bf16* row = logits + int64_t(b) * ld;
+  const bf16* row = logits + int64_t(r) * ld;
   float best = -INFINITY;
   int bi = -1;
   for (int v = tid; v < V; v += SEL_THREADS) {   // increasing v per thread: strict '>' keeps the lowest index
@@ -267,13 +281,94 @@ __global__ void __launch_bounds__(SEL_THREADS) greedy_select_kernel(
       const int oi = s_idx[w];
       if (argmax_better(ov, oi, best, bi)) { best = ov; bi = oi; }
     }
-    const int fin = finished[b];
+    const int fin = SLOTS ? 0 : finished[b];
     const int64_t tok = fin ? pad : int64_t(bi);
     if (len < ld_hist) history[int64_t(b) * ld_hist + len] = tok;
     next_ids[b] = tok;
     length[b] = len + 1;
     positions[b] += 1;
-    if (tok == eos) finished[b] = 1;
+    if (tok == eos || (SLOTS && len + 1 == limit[b])) finished[b] = 1;
+  }
+}
+
+__global__ void __launch_bounds__(SEL_THREADS) greedy_select_kernel(
+    const bf16* __restrict__ logits, int64_t ld, int V, int64_t* __restrict__ history, int64_t ld_hist,
+    int32_t* __restrict__ length, int64_t* __restrict__ positions, int64_t* __restrict__ next_ids,
+    int32_t* __restrict__ finished, float penalty, int ngram, int64_t eos, int64_t pad) {
+  greedy_select_row<false>(logits, ld, V, history, ld_hist, length, positions, next_ids, finished, nullptr, penalty,
+                           ngram, eos, pad, blockIdx.x, blockIdx.x);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// continuous batching: slot-addressed admission state, K/V scatter of a packed prefill, slot-aware selection
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int ADMIT_MAX = TN_ADMIT_MAX;       // documents per admission launch
+constexpr int SEL_MAX_MAP = TN_SELECT_MAX_MAP;  // rows of an explicit row -> slot map
+
+// The admission table travels in the launch's parameter block (2 KB), so the entry points validate every slot and
+// length on the host and admission needs no host-to-device copy.
+struct AdmitTable {
+  int n;
+  int src_row[ADMIT_MAX], slot[ADMIT_MAX], len[ADMIT_MAX], limit[ADMIT_MAX];
+};
+
+struct SlotMap {
+  int use_map;                       // 0: row r is slot r
+  int slot[SEL_MAX_MAP];
+};
+
+__global__ void __launch_bounds__(SEL_THREADS, 1) greedy_select_slots_kernel(
+    const bf16* __restrict__ logits, int64_t ld, int V, int64_t* __restrict__ history, int64_t ld_hist,
+    int32_t* __restrict__ length, int64_t* __restrict__ positions, int64_t* __restrict__ next_ids,
+    int32_t* __restrict__ finished, const int32_t* __restrict__ limit, float penalty, int ngram, int64_t eos,
+    int64_t pad, const SlotMap map) {
+  const int r = blockIdx.x;
+  greedy_select_row<true>(logits, ld, V, history, ld_hist, length, positions, next_ids, finished, limit, penalty, ngram,
+                          eos, pad, r, map.use_map ? map.slot[r] : r);
+}
+
+// grid (longest document, documents): row t of document j -> cache row t of slot j, 16-byte copies
+__global__ void kv_scatter_kernel(const bf16* __restrict__ K, int64_t ldk, const bf16* __restrict__ V, int64_t ldv,
+                                  bf16* __restrict__ Kc, bf16* __restrict__ Vc, int64_t ld_tok, int64_t ld_batch,
+                                  const AdmitTable tab, int width) {
+  const int t = blockIdx.x, j = blockIdx.y;
+  if (t >= tab.len[j]) return;
+  const int64_t src = int64_t(tab.src_row[j]) + t;
+  const int64_t dst = int64_t(tab.slot[j]) * ld_batch + int64_t(t) * ld_tok;
+  for (int i = threadIdx.x; i < width / 8; i += blockDim.x) {
+    reinterpret_cast<uint4*>(Kc + dst)[i] = reinterpret_cast<const uint4*>(K + src * ldk)[i];
+    reinterpret_cast<uint4*>(Vc + dst)[i] = reinterpret_cast<const uint4*>(V + src * ldv)[i];
+  }
+}
+
+constexpr int ADMIT_THREADS = 256;
+
+// one CTA per admitted document: its slot's decoding state and the prompt ids of its history
+__global__ void __launch_bounds__(ADMIT_THREADS) slot_admit_kernel(
+    const AdmitTable tab, const int64_t* __restrict__ ids, const int32_t* __restrict__ doc_ids,
+    const int64_t* __restrict__ position_ids, int64_t* __restrict__ history, int64_t ld_hist,
+    int32_t* __restrict__ kv_start, int32_t* __restrict__ kv_end, int64_t* __restrict__ positions,
+    int32_t* __restrict__ finished, int32_t* __restrict__ limit) {
+  __shared__ int s_start[ADMIT_THREADS / 32];
+  const int j = blockIdx.x, tid = threadIdx.x;
+  const int src = tab.src_row[j], b = tab.slot[j], T = tab.len[j];
+  const int32_t* doc = doc_ids + src;
+  const int32_t last = doc[T - 1];
+  int start = 0;                       // first row of the last document = 1 + the last row outside it
+  for (int t = tid; t < T; t += ADMIT_THREADS) {
+    if (doc[t] != last) start = t + 1;
+    history[int64_t(b) * ld_hist + t] = ids[src + t];
+  }
+  start = __reduce_max_sync(0xffffffffu, start);
+  if ((tid & 31) == 0) s_start[tid >> 5] = start;
+  __syncthreads();
+  if (tid == 0) {
+    for (int w = 1; w < ADMIT_THREADS / 32; ++w) start = max(start, s_start[w]);
+    kv_start[b] = start;
+    kv_end[b] = T;
+    positions[b] = position_ids[src + T - 1];
+    finished[b] = 0;
+    limit[b] = tab.limit[j];
   }
 }
 
@@ -358,6 +453,112 @@ extern "C" int tn_greedy_select_bf16(const void* logits, int64_t ld, int B, int 
   greedy_select_kernel<<<B, SEL_THREADS, smem, stream>>>(static_cast<const bf16*>(logits), ld, V, history, ld_hist,
                                                          length, positions, next_ids, finished, repetition_penalty,
                                                          no_repeat_ngram_size, eos, pad);
+  TN_CHECK_CUDA(cudaGetLastError());
+  return TN_OK;
+}
+
+extern "C" int tn_greedy_select_slots_bf16(const void* logits, int64_t ld, int n_rows, const int32_t* row_slot, int B,
+                                           int V, int64_t* history, int64_t ld_hist, int32_t* length, int64_t* positions,
+                                           int64_t* next_ids, int32_t* finished, const int32_t* limit,
+                                           float repetition_penalty, int no_repeat_ngram_size, int64_t eos, int64_t pad,
+                                           tn_stream_t stream_) {
+  clear_error();
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  TN_REQUIRE(logits && history && length && positions && next_ids && finished && limit,
+             "tn_greedy_select_slots_bf16: null pointer");
+  TN_REQUIRE(n_rows > 0 && B > 0 && V > 0 && ld >= V && ld_hist > 0, "tn_greedy_select_slots_bf16: bad dims n_rows=%d "
+             "B=%d V=%d", n_rows, B, V);
+  TN_REQUIRE(row_slot || n_rows == B, "tn_greedy_select_slots_bf16: bad dims: without a row -> slot map n_rows (%d) "
+             "must equal B (%d)", n_rows, B);
+  TN_REQUIRE(!row_slot || n_rows <= SEL_MAX_MAP, "tn_greedy_select_slots_bf16: at most %d mapped rows, got %d",
+             SEL_MAX_MAP, n_rows);
+  TN_REQUIRE(repetition_penalty > 0.f, "tn_greedy_select_slots_bf16: repetition_penalty must be > 0");
+  TN_REQUIRE(no_repeat_ngram_size >= 0, "tn_greedy_select_slots_bf16: no_repeat_ngram_size must be >= 0");
+  const size_t smem = size_t(2) * ((V + 31) / 32) * sizeof(uint32_t);
+  TN_REQUIRE(smem <= 200 * 1024, "tn_greedy_select_slots_bf16: vocabulary of %d too large for the shared-memory bitmaps",
+             V);
+  SlotMap map{};
+  map.use_map = row_slot != nullptr;
+  for (int r = 0; row_slot && r < n_rows; ++r) {   // the map is host memory: checked here, passed by value
+    TN_REQUIRE(row_slot[r] >= 0 && row_slot[r] < B, "tn_greedy_select_slots_bf16: slot %d out of range [0, %d)",
+               row_slot[r], B);
+    for (int q = 0; q < r; ++q)
+      TN_REQUIRE(row_slot[q] != row_slot[r], "tn_greedy_select_slots_bf16: slot %d named twice", row_slot[r]);
+    map.slot[r] = row_slot[r];
+  }
+  static bool configured = false;
+  if (!configured) {
+    TN_CHECK_CUDA(cudaFuncSetAttribute(greedy_select_slots_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       200 * 1024));
+    configured = true;
+  }
+  greedy_select_slots_kernel<<<n_rows, SEL_THREADS, smem, stream>>>(
+      static_cast<const bf16*>(logits), ld, V, history, ld_hist, length, positions, next_ids, finished, limit,
+      repetition_penalty, no_repeat_ngram_size, eos, pad, map);
+  TN_CHECK_CUDA(cudaGetLastError());
+  return TN_OK;
+}
+
+// docs: host [n_docs][4] int32 = (src_row, slot, len, limit); checked against the cache shape, returned by value
+static int admit_table(const char* fn, const int32_t* docs, int n_docs, int B, int S_cap, int64_t n_src_rows,
+                       AdmitTable* tab, int* max_len) {
+  TN_REQUIRE(n_docs > 0 && n_docs <= ADMIT_MAX, "%s: bad dims: %d documents (1..%d per launch)", fn, n_docs, ADMIT_MAX);
+  tab->n = n_docs;
+  *max_len = 0;
+  for (int j = 0; j < n_docs; ++j) {
+    const int src = docs[4 * j], slot = docs[4 * j + 1], len = docs[4 * j + 2], lim = docs[4 * j + 3];
+    TN_REQUIRE(slot >= 0 && slot < B, "%s: slot %d out of range [0, %d)", fn, slot, B);
+    for (int q = 0; q < j; ++q) TN_REQUIRE(tab->slot[q] != slot, "%s: slot %d named twice", fn, slot);
+    TN_REQUIRE(len > 0 && len <= S_cap, "%s: bad dims: document of %d rows for a cache of %d", fn, len, S_cap);
+    TN_REQUIRE(src >= 0 && int64_t(src) + len <= n_src_rows, "%s: document rows [%d, %d) outside the %lld source rows",
+               fn, src, src + len, (long long)n_src_rows);
+    TN_REQUIRE(lim > len && lim <= S_cap, "%s: limit %d must be in (%d, %d]", fn, lim, len, S_cap);
+    tab->src_row[j] = src; tab->slot[j] = slot; tab->len[j] = len; tab->limit[j] = lim;
+    if (len > *max_len) *max_len = len;
+  }
+  return TN_OK;
+}
+
+extern "C" int tn_kv_scatter_bf16(const void* K, int64_t ldk, const void* V, int64_t ldv, int64_t n_src_rows,
+                                  void* K_cache, void* V_cache, int64_t ld_tok, int64_t ld_batch, const int32_t* docs,
+                                  int n_docs, int B, int S_cap, int width, tn_stream_t stream_) {
+  clear_error();
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  TN_REQUIRE(K && V && K_cache && V_cache && docs, "tn_kv_scatter_bf16: null pointer");
+  TN_REQUIRE(B > 0 && S_cap > 0 && width > 0 && width % 8 == 0 && n_src_rows > 0,
+             "tn_kv_scatter_bf16: bad dims B=%d S_cap=%d width=%d", B, S_cap, width);
+  TN_REQUIRE(ldk % 8 == 0 && ldv % 8 == 0 && ld_tok % 8 == 0 && ld_batch % 8 == 0 && ldk >= width && ldv >= width &&
+                 ld_tok >= width && ld_batch >= ld_tok * S_cap, "tn_kv_scatter_bf16: bad strides");
+  TN_REQUIRE(((uintptr_t(K) | uintptr_t(V) | uintptr_t(K_cache) | uintptr_t(V_cache)) & 15) == 0,
+             "tn_kv_scatter_bf16: pointers must be 16-byte aligned");
+  AdmitTable tab{};
+  int max_len = 0;
+  const int rc = admit_table("tn_kv_scatter_bf16", docs, n_docs, B, S_cap, n_src_rows, &tab, &max_len);
+  if (rc != TN_OK) return rc;
+  kv_scatter_kernel<<<dim3(max_len, n_docs), 128, 0, stream>>>(
+      static_cast<const bf16*>(K), ldk, static_cast<const bf16*>(V), ldv, static_cast<bf16*>(K_cache),
+      static_cast<bf16*>(V_cache), ld_tok, ld_batch, tab, width);
+  TN_CHECK_CUDA(cudaGetLastError());
+  return TN_OK;
+}
+
+extern "C" int tn_slot_admit(const int32_t* docs, int n_docs, const int64_t* ids, const int32_t* doc_ids,
+                             const int64_t* position_ids, int64_t n_src_rows, int64_t* history, int64_t ld_hist,
+                             int32_t* kv_start, int32_t* kv_end, int64_t* positions, int32_t* finished, int32_t* limit,
+                             int B, tn_stream_t stream_) {
+  clear_error();
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  TN_REQUIRE(docs && ids && doc_ids && position_ids && history && kv_start && kv_end && positions && finished && limit,
+             "tn_slot_admit: null pointer");
+  TN_REQUIRE(B > 0 && ld_hist > 0 && n_src_rows > 0, "tn_slot_admit: bad dims B=%d ld_hist=%lld", B,
+             (long long)ld_hist);
+  AdmitTable tab{};
+  int max_len = 0;
+  const int rc = admit_table("tn_slot_admit", docs, n_docs, B, int(ld_hist < INT32_MAX ? ld_hist : INT32_MAX), n_src_rows,
+                             &tab, &max_len);
+  if (rc != TN_OK) return rc;
+  slot_admit_kernel<<<n_docs, ADMIT_THREADS, 0, stream>>>(tab, ids, doc_ids, position_ids, history, ld_hist, kv_start,
+                                                          kv_end, positions, finished, limit);
   TN_CHECK_CUDA(cudaGetLastError());
   return TN_OK;
 }

@@ -11,7 +11,11 @@ repetition_penalty, no_repeat_ngram_size, max_new_tokens, ...)` on left-padded p
            attention (tn_attn_decode_bf16), then lm_head and the greedy selection kernel (tn_greedy_select_bf16:
            repetition penalty, no-repeat-ngram ban, argmax, pad after eos), all lengths and positions on the device;
   generate prefill, one eager decode step, then the decode step captured once in a CUDA graph and replayed per token,
-           with one host sync per step to read the finished flags and the NaN flag.
+           with one host sync per step to read the finished flags and the NaN flag;
+  generate_many
+           continuous batching over many prompts: a cache of B slots, finished rows refilled with the next prompts
+           (packed prefill into chosen slots: tn_kv_scatter_bf16, tn_slot_admit) while the captured decode step keeps
+           replaying (tn_greedy_select_slots_bf16 holds finished and idle slots still).
 
 The new tokens belong to the last document of each row: the decode query of row b attends to cache rows
 [kv_start[b], kv_end[b]) with kv_start[b] the first position of the row's last document in the prompt's attention_mask
@@ -324,3 +328,237 @@ def generate(model, input_ids, input_features=None, attention_mask=None, positio
         if n == max_new and nan_flag is not None:
             done()
     return cache.history[:, :T + n].clone()
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# continuous batching
+# ---------------------------------------------------------------------------------------------------------------
+_ALIGN = 128            # rows of one attention q block: each admitted prompt starts on a block boundary
+_MIN_PACKED_ROWS = 256  # a packed prefill row always takes the fused-QKV path (ops.qkv_fusable), alone or not
+_ADMIT_MAX = 128        # documents per admission launch (TN_ADMIT_MAX)
+
+
+class _Prompt:
+    """One utterance of generate_many, validated and on the model's device."""
+
+    def __init__(self, index, p, audio, max_len, budget, dev):
+        if not isinstance(p, dict) or "input_ids" not in p:
+            raise TouchNetB200Error(f"generate_many: prompt {index} must be a dict with 'input_ids'")
+        unknown = sorted(set(p) - {"input_ids", "input_features", "attention_mask", "position_ids"})
+        if unknown:
+            raise TouchNetB200Error(f"generate_many: prompt {index}: unsupported keys {unknown}")
+        ids = torch.as_tensor(p["input_ids"])
+        if ids.dim() != 1 or ids.numel() == 0:
+            raise TouchNetB200Error(f"generate_many: prompt {index}: input_ids must be a non-empty 1-D tensor")
+        T = ids.numel()
+        if T > max_len:
+            raise TouchNetB200Error(f"generate_many: prompt {index} has {T} tokens, more than max_prompt_length "
+                                    f"{max_len}")
+        feats = p.get("input_features")
+        if feats is not None:
+            if audio is None:
+                raise TouchNetB200Error("generate_many: unsupported arguments ['input_features'] (a text-only model)")
+            if feats.dim() != 2 or feats.shape[0] != T:
+                raise TouchNetB200Error(f"generate_many: prompt {index}: input_features must be [T, F] with T = {T}")
+        mask = p.get("attention_mask")
+        mask = torch.ones(T, dtype=torch.int64, device=dev) if mask is None else mask.to(dev, torch.int64)
+        _check_mask(mask.reshape(1, -1), 1, T)
+        pos = p.get("position_ids")
+        if pos is None:                   # as prefill: cumsum of the mask, 1 at padding
+            m = (mask != 0).to(torch.int64)
+            pos = (m.cumsum(-1) - 1).masked_fill_(m == 0, 1)
+        elif tuple(pos.shape) != (T,):
+            raise TouchNetB200Error(f"generate_many: prompt {index}: position_ids must be [{T}]")
+        self.index, self.T, self.budget = index, T, budget
+        self.ids = ids.to(dev, torch.int64)
+        self.feats = None if feats is None else feats.to(dev)
+        self.mask, self.pos = mask, pos.to(dev, torch.int64)
+
+
+def _admit(model, cache: B200KVCache, limit: torch.Tensor, w: _Weights, batch, pad: int, select) -> None:
+    """Prefill `batch` [(slot, _Prompt)] into their slots as ONE packed row of documents and select each one's first
+    token.  Prompt j occupies rows [o_j, o_j + T_j), o_j a multiple of 128; its documents are its runs of equal
+    attention_mask values (padding included: never attended by the new tokens), relabelled o_j + run index so the row's
+    ids are non-decreasing and non-zero; the gap rows after it continue its last document (ids pad, features zero),
+    so every 128-row q block holds rows of one prompt and sees the K/V blocks it sees when prefilled alone.  Slots not
+    in `batch` are not touched."""
+    lm, audio = _parts(model)
+    dev = cache.data.device
+    offs, o = [], 0
+    for _, p in batch:
+        offs.append(o)
+        o += -(-p.T // _ALIGN) * _ALIGN
+    n = max(o, _MIN_PACKED_ROWS)
+    ids = torch.empty(n, dtype=torch.int64, device=dev)
+    doc = torch.empty(n, dtype=torch.int64, device=dev)
+    pos = torch.zeros(n, dtype=torch.int64, device=dev)
+    any_feats = any(p.feats is not None and p.T != 1 for _, p in batch)
+    feats = None
+    if any_feats:
+        width = next(p.feats.shape[1] for _, p in batch if p.feats is not None)
+        feats = torch.zeros((n, width), dtype=BF16, device=dev)
+    docs = []
+    for j, ((slot, p), o0) in enumerate(zip(batch, offs)):
+        end = offs[j + 1] if j + 1 < len(batch) else n
+        m = p.mask
+        runs = torch.cat([m.new_zeros(1), (m[1:] != m[:-1]).to(torch.int64).cumsum(0)]) + (o0 + 1)
+        doc[o0:o0 + p.T] = runs
+        doc[o0 + p.T:end] = runs[-1]
+        ids[o0:o0 + p.T] = p.ids
+        ids[o0 + p.T:end] = pad
+        pos[o0:o0 + p.T] = p.pos
+        if feats is not None and p.feats is not None and p.T != 1:     # as generate: no projector on a 1-token prompt
+            feats[o0:o0 + p.T] = p.feats.to(BF16)
+        docs.append((o0, slot, p.T, p.T + p.budget))
+    x = _prompt_embeds(model, ids.view(1, n), None if feats is None else feats.view(1, n, -1), w)
+    plan = ops.AttnPlan(doc.view(1, n))
+    cos, sin = ops.rope_table(pos.view(1, n), w.inv_freq, w.rope_scaling)
+    ops.slot_admit(docs, ids, plan.doc.view(-1), pos, cache.history, cache.kv_start, cache.kv_end, cache.positions,
+                   cache.finished, limit)
+    H, KV, hd = cache.H, cache.KV, cache.hd
+    scale = 1.0 / math.sqrt(hd)
+    for i, lw in enumerate(w.layers):
+        kc, vc = cache.layer(i)
+
+        def attend(q, k, v, kc=kc, vc=vc):
+            ops.kv_scatter(k, v, kc, vc, docs)
+            o, lse = ops.attn_fwd(q, k, v, plan, H, KV, scale)
+            return o, lse, k, v
+
+        x, _ = ops.block_forward(x, *lw, cos, sin, H, KV, w.eps, hd, attend, need_gu=False)
+    last = torch.tensor([o0 + p.T - 1 for (_, p), o0 in zip(batch, offs)], dtype=torch.int64).to(dev)
+    select(_logits_last(w, x.index_select(0, last)), [slot for slot, _ in batch])
+
+
+def generate_many(model, prompts, *, batch_size, max_new_tokens, eos_token_id, pad_token_id, repetition_penalty=1.0,
+                  no_repeat_ngram_size=0, max_prompt_length=None, cuda_graph: bool = True, stats: Optional[dict] = None):
+    """Greedy decoding of many prompts with continuous batching: a cache of `batch_size` slots; when a slot's row
+    finishes (eos or its token budget), its generated ids are copied out and the next prompt is prefilled into that slot
+    while the other slots keep decoding.  Per prompt, the result is what `generate` returns for that prompt alone
+    (HF greedy with the same processors), as a 1-D int64 tensor of the generated ids (eos included if reached, no
+    padding); the list is in input order.
+
+    prompts          iterable of dicts: input_ids [T], optional input_features [T, F] (TouchAudio), attention_mask [T]
+                     (doc ids or 0/1, last document rule of `generate`), position_ids [T]
+    max_new_tokens   an int, or one budget per prompt
+    max_prompt_length  the longest prompt to expect (default: the longest of `prompts` when it is a sequence)
+    cuda_graph       False runs every decode step eagerly (the captured step computes the same bits)
+    stats            if a dict, receives decode_steps, admissions and, on CUDA, admission_events (pairs of CUDA events
+                     around each admission prefill)"""
+    budgets = None
+    if isinstance(max_new_tokens, (list, tuple)) or (torch.is_tensor(max_new_tokens) and max_new_tokens.dim() == 1):
+        budgets = [int(b) for b in max_new_tokens]
+        if not budgets:
+            raise TouchNetB200Error("generate_many: max_new_tokens is an empty sequence")
+        bad = [b for b in budgets if b < 1]
+        if bad:
+            raise TouchNetB200Error(f"generate: max_new_tokens must be >= 1, got {bad[0]}")
+        max_budget = max(budgets)
+    else:
+        max_budget = int(max_new_tokens)
+    _validate(max_budget, eos_token_id, pad_token_id, repetition_penalty, no_repeat_ngram_size, False, 1, {})
+    _check_scope(model)
+    B = int(batch_size)
+    if B < 1:
+        raise TouchNetB200Error(f"generate_many: batch_size must be >= 1, got {batch_size}")
+    if hasattr(prompts, "__len__") and hasattr(prompts, "__getitem__") and not isinstance(prompts, dict):
+        prompts = list(prompts)
+        if budgets is not None and len(budgets) != len(prompts):
+            raise TouchNetB200Error(f"generate_many: {len(budgets)} budgets for {len(prompts)} prompts")
+        if not prompts:
+            return []
+        if max_prompt_length is None:
+            max_prompt_length = max(1, max(torch.as_tensor(p["input_ids"]).numel() if isinstance(p, dict) and
+                                           "input_ids" in p else 0 for p in prompts))
+    elif max_prompt_length is None:
+        raise TouchNetB200Error("generate_many: max_prompt_length is required when prompts is not a sequence")
+    max_len = int(max_prompt_length)
+    if max_len < 1:
+        raise TouchNetB200Error(f"generate_many: max_prompt_length must be >= 1, got {max_prompt_length}")
+    eos, pad = int(eos_token_id), int(pad_token_id)
+    lm, audio = _parts(model)
+    dev = lm.lm_head.weight.device
+    it = iter(prompts)
+    results: dict = {}
+    slot_prompt: list = [None] * B            # the _Prompt decoding in each slot, None = idle
+    count = 0
+    with torch.no_grad():
+        w = _Weights(lm)
+        cache = B200KVCache(model, B, max_len + max_budget, device=dev)
+        limit = torch.zeros(B, dtype=torch.int32, device=dev)
+        cache.finished.fill_(1)               # every slot starts idle
+        nan_flag = None if audio is None else audio._nan_flag
+        admission_events = []
+        admissions = 0
+
+        def select_decode(logits):
+            ops.greedy_select_slots(logits, cache.history, cache.kv_end, cache.positions, cache.next_ids,
+                                    cache.finished, limit, float(repetition_penalty), int(no_repeat_ngram_size), eos,
+                                    pad)
+
+        def select_admitted(logits, slots):
+            ops.greedy_select_slots(logits, cache.history, cache.kv_end, cache.positions, cache.next_ids,
+                                    cache.finished, limit, float(repetition_penalty), int(no_repeat_ngram_size), eos,
+                                    pad, row_slot=slots)
+
+        def admit(free) -> None:
+            nonlocal count, admissions
+            batch = []
+            for slot in free:
+                try:
+                    p = next(it)
+                except StopIteration:
+                    break
+                if budgets is not None and count >= len(budgets):
+                    raise TouchNetB200Error("generate_many: more prompts than budgets")
+                budget = budgets[count] if budgets is not None else max_budget
+                batch.append((slot, _Prompt(count, p, audio, max_len, budget, dev)))
+                count += 1
+            for i in range(0, len(batch), _ADMIT_MAX):
+                chunk = batch[i:i + _ADMIT_MAX]
+                ev = None
+                if stats is not None and dev.type == "cuda":
+                    ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
+                    ev[0].record()
+                _admit(model, cache, limit, w, chunk, pad, select_admitted)
+                admissions += 1
+                if ev is not None:
+                    ev[1].record()
+                    admission_events.append(ev)
+                for slot, p in chunk:
+                    slot_prompt[slot] = p
+
+        def step() -> None:
+            select_decode(decode_step(model, cache, weights=w))
+
+        admit(list(range(B)))
+        graph, steps = None, 0
+        while any(p is not None for p in slot_prompt):
+            if graph is None and steps >= 1 and cuda_graph and dev.type == "cuda":
+                graph = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(graph):
+                    step()
+            if graph is not None:
+                graph.replay()
+            else:
+                step()                        # the first decode step runs eagerly
+            steps += 1
+            flags = torch.cat([cache.finished, cache.kv_end] + ([] if nan_flag is None else [nan_flag.reshape(1)]))
+            vals = flags.tolist()             # the one host sync per step
+            if nan_flag is not None and vals[-1] != 0:
+                nan_flag.zero_()
+                raise ValueError("NaN in data.")
+            free = []
+            for s in range(B):
+                p = slot_prompt[s]
+                if p is not None and vals[s] != 0:
+                    results[p.index] = cache.history[s, p.T:vals[B + s]].clone()
+                    slot_prompt[s] = None
+                    free.append(s)
+            if free:
+                admit(free)
+        if stats is not None:
+            stats.update(decode_steps=steps, admissions=admissions, admission_events=admission_events)
+    if budgets is not None and count != len(budgets):
+        raise TouchNetB200Error(f"generate_many: {len(budgets)} budgets for {count} prompts")
+    return [results[i] for i in range(count)]

@@ -401,6 +401,11 @@ class B200LlamaForCausalLM(nn.Module):
         kwargs.pop("input_features", None)
         return generation.generate(self, input_ids, None, attention_mask, position_ids, **kwargs)
 
+    def generate_many(self, prompts, **kwargs: Any):
+        """Greedy decoding of many prompts with continuous batching (see generation.generate_many)."""
+        from . import generation
+        return generation.generate_many(self, prompts, **kwargs)
+
 
 class B200TouchAudioForCausalLM(nn.Module):
     """ref: touchnet/models/touch_audio/modeling_touch_audio.py:19-152 (a.k.a. LlamaForASR, docs/TouchAudioForCausalLM.md)."""
@@ -519,6 +524,12 @@ class B200TouchAudioForCausalLM(nn.Module):
         `generate` semantics, the audio features projected into the prompt only (see generation.generate)."""
         from . import generation
         return generation.generate(self, input_ids, input_features, attention_mask, position_ids, **kwargs)
+
+    def generate_many(self, prompts, **kwargs: Any):
+        """The evaluation call over a whole test set with continuous batching: finished rows are refilled with the next
+        utterances while the others keep decoding (see generation.generate_many)."""
+        from . import generation
+        return generation.generate_many(self, prompts, **kwargs)
 
 
 __all__ = ["B200LlamaForCausalLM", "B200TouchAudioForCausalLM", "B200LlamaModel", "B200DecoderLayer", "B200RMSNorm",

@@ -421,6 +421,50 @@ def greedy_select(logits, history, length, positions, next_ids, finished, repeti
               float(repetition_penalty), int(no_repeat_ngram_size), int(eos), int(pad), _st())
 
 
+def _host_i32(rows) -> torch.Tensor:
+    """A small int32 table in host memory (the continuous-batching entry points copy it into the launch)."""
+    return torch.tensor(rows, dtype=torch.int32).reshape(-1).contiguous()
+
+
+def kv_scatter(k, v, k_cache, v_cache, docs):
+    """Cache rows [0, len) of slot `slot` <- rows [src_row, src_row + len) of k / v [rows, KV*128], for each
+    (src_row, slot, len, limit) in `docs` (a list; limit is not used here)."""
+    _chk(k, "k", BF16); _chk(v, "v", BF16); _chk(k_cache, "k_cache", BF16)
+    B, S_cap, width = k_cache.shape
+    assert k_cache.stride() == v_cache.stride() and k.shape[1] == width and k.stride(1) == 1 and v.stride(1) == 1
+    tab = _host_i32(docs)
+    _lib.call("tn_kv_scatter_bf16", k.data_ptr(), k.stride(0), v.data_ptr(), v.stride(0), k.shape[0], k_cache.data_ptr(),
+              v_cache.data_ptr(), k_cache.stride(1), k_cache.stride(0), tab.data_ptr(), len(docs), B, S_cap, width, _st())
+
+
+def slot_admit(docs, ids, doc_ids, position_ids, history, kv_start, kv_end, positions, finished, limit):
+    """Decoding state of the slots named in `docs` [(src_row, slot, len, limit)] from the packed prompt row (ids /
+    position_ids int64, doc_ids int32, all [rows]); other slots are not touched."""
+    _chk(ids, "ids", torch.int64); _chk(doc_ids, "doc_ids", torch.int32); _chk(position_ids, "position_ids", torch.int64)
+    _chk(history, "history", torch.int64); _chk(kv_start, "kv_start", torch.int32); _chk(limit, "limit", torch.int32)
+    assert history.stride(1) == 1
+    tab = _host_i32(docs)
+    _lib.call("tn_slot_admit", tab.data_ptr(), len(docs), ids.data_ptr(), doc_ids.data_ptr(), position_ids.data_ptr(),
+              ids.numel(), history.data_ptr(), history.stride(0), kv_start.data_ptr(), kv_end.data_ptr(),
+              positions.data_ptr(), finished.data_ptr(), limit.data_ptr(), history.shape[0], _st())
+
+
+def greedy_select_slots(logits, history, length, positions, next_ids, finished, limit, repetition_penalty: float,
+                        no_repeat_ngram_size: int, eos: int, pad: int, row_slot=None):
+    """greedy_select over cache slots: logits row r selects for slot row_slot[r] (a list; None = slot r).  Finished or
+    idle slots do not advance (pad in next_ids); a slot finishes on eos or when its length reaches limit."""
+    _chk(logits, "logits", BF16); _chk(history, "history", torch.int64); _chk(length, "length", torch.int32)
+    _chk(positions, "positions", torch.int64); _chk(next_ids, "next_ids", torch.int64)
+    _chk(finished, "finished", torch.int32); _chk(limit, "limit", torch.int32)
+    n, V = logits.shape
+    assert logits.stride(1) == 1 and history.stride(1) == 1
+    tab = None if row_slot is None else _host_i32(row_slot)
+    _lib.call("tn_greedy_select_slots_bf16", logits.data_ptr(), logits.stride(0), n, None if tab is None else tab.data_ptr(),
+              history.shape[0], V, history.data_ptr(), history.stride(0), length.data_ptr(), positions.data_ptr(),
+              next_ids.data_ptr(), finished.data_ptr(), limit.data_ptr(), float(repetition_penalty),
+              int(no_repeat_ngram_size), int(eos), int(pad), _st())
+
+
 def embed_add(input_ids: Optional[torch.Tensor], embed: Optional[torch.Tensor], proj: Optional[torch.Tensor],
               rows: int, d: int, nan_flag: Optional[torch.Tensor] = None):
     """E = embed[input_ids] + proj (either may be None)."""
