@@ -36,8 +36,8 @@ def test_slot_entry_points_reject_bad_arguments():
     kv = lambda K=p, ldk=128, docs=ok, n=1, ld_batch=128 * 64, rows=64: (    # noqa: E731
         K, ldk, p, 128, rows, p, p, 128, ld_batch, docs, n, 4, 64, 128, None)
     adm = lambda docs=ok, n=1, ids=p, B=4: (docs, n, ids, p, p, 64, p, 64, p, p, p, p, p, B, None)   # noqa: E731
-    sel = lambda logits=p, n=4, m=None, B=4, ld=64, pen=1.5, ng=2: (                                  # noqa: E731
-        logits, ld, n, m, B, 64, p, 16, p, p, p, p, p, pen, ng, 1, 0, None)
+    sel = lambda logits=p, n=4, m=None, B=4, ld=64, V=64, pen=1.5, ng=2: (                            # noqa: E731
+        logits, ld, n, m, B, V, p, 16, p, p, p, p, p, pen, ng, 1, 0, None)
     bad_calls = [
         ("tn_kv_scatter_bf16", kv(K=None), "null"),
         ("tn_kv_scatter_bf16", kv(n=0), "bad dims"),
@@ -61,6 +61,7 @@ def test_slot_entry_points_reject_bad_arguments():
         ("tn_greedy_select_slots_bf16", sel(n=300, m=ctypes.addressof(map_arr), B=400), "at most"),
         ("tn_greedy_select_slots_bf16", sel(pen=0.0), "repetition_penalty"),
         ("tn_greedy_select_slots_bf16", sel(ng=-1), "no_repeat_ngram_size"),
+        ("tn_greedy_select_slots_bf16", sel(ld=1 << 23, V=1 << 23, pen=1.0, ng=0), "too large"),
     ]
     for name, args, needle in bad_calls:
         with pytest.raises(_lib.TouchNetB200Error, match=needle):

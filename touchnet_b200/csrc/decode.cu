@@ -186,24 +186,29 @@ __global__ void __launch_bounds__(ATT_HD) attn_decode_merge_kernel(const float* 
 // ---------------------------------------------------------------------------------------------------------------
 // cache append: rows [end[b] - T_new, end[b]) of batch row b <- source rows b*T_new .. b*T_new + T_new - 1
 // ---------------------------------------------------------------------------------------------------------------
-__global__ void kv_append_kernel(const bf16* __restrict__ K, int64_t ldk, const bf16* __restrict__ V, int64_t ldv,
-                                 bf16* __restrict__ Kc, bf16* __restrict__ Vc, int64_t ld_tok, int64_t ld_batch,
-                                 const int32_t* __restrict__ row_end, int T_new, int S_cap, int width) {
-  const int t = blockIdx.x, b = blockIdx.y;
-  const int row = row_end[b] - T_new + t;
-  if (row < 0 || row >= S_cap) return;
-  const int64_t src = int64_t(b) * T_new + t;
-  const int64_t dst = int64_t(b) * ld_batch + int64_t(row) * ld_tok;
+// row `src` of K / V -> element offset `dst` of Kc / Vc: `width` bf16 in 16-byte copies over the CTA's threads
+__device__ __forceinline__ void copy_kv_row(const bf16* K, int64_t ldk, const bf16* V, int64_t ldv, bf16* Kc, bf16* Vc,
+                                            int64_t src, int64_t dst, int width) {
   for (int i = threadIdx.x; i < width / 8; i += blockDim.x) {
     reinterpret_cast<uint4*>(Kc + dst)[i] = reinterpret_cast<const uint4*>(K + src * ldk)[i];
     reinterpret_cast<uint4*>(Vc + dst)[i] = reinterpret_cast<const uint4*>(V + src * ldv)[i];
   }
 }
 
+__global__ void kv_append_kernel(const bf16* __restrict__ K, int64_t ldk, const bf16* __restrict__ V, int64_t ldv,
+                                 bf16* __restrict__ Kc, bf16* __restrict__ Vc, int64_t ld_tok, int64_t ld_batch,
+                                 const int32_t* __restrict__ row_end, int T_new, int S_cap, int width) {
+  const int t = blockIdx.x, b = blockIdx.y;
+  const int row = row_end[b] - T_new + t;
+  if (row < 0 || row >= S_cap) return;
+  copy_kv_row(K, ldk, V, ldv, Kc, Vc, int64_t(b) * T_new + t, int64_t(b) * ld_batch + int64_t(row) * ld_tok, width);
+}
+
 // ---------------------------------------------------------------------------------------------------------------
 // greedy selection with HF's repetition penalty and no-repeat-ngram processors, one CTA per batch row
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int SEL_THREADS = 1024;
+constexpr size_t SEL_MAX_SMEM = 204800;   // 200 KB: the most dynamic shared memory a selection CTA's bitmaps may take
 
 // torch.argmax order: NaN above every number, then the larger value, then the lower index; index -1 = no candidate
 __device__ __forceinline__ bool argmax_better(float x, int i, float best, int bi) {
@@ -333,12 +338,8 @@ __global__ void kv_scatter_kernel(const bf16* __restrict__ K, int64_t ldk, const
                                   const AdmitTable tab, int width) {
   const int t = blockIdx.x, j = blockIdx.y;
   if (t >= tab.len[j]) return;
-  const int64_t src = int64_t(tab.src_row[j]) + t;
-  const int64_t dst = int64_t(tab.slot[j]) * ld_batch + int64_t(t) * ld_tok;
-  for (int i = threadIdx.x; i < width / 8; i += blockDim.x) {
-    reinterpret_cast<uint4*>(Kc + dst)[i] = reinterpret_cast<const uint4*>(K + src * ldk)[i];
-    reinterpret_cast<uint4*>(Vc + dst)[i] = reinterpret_cast<const uint4*>(V + src * ldv)[i];
-  }
+  copy_kv_row(K, ldk, V, ldv, Kc, Vc, int64_t(tab.src_row[j]) + t,
+              int64_t(tab.slot[j]) * ld_batch + int64_t(t) * ld_tok, width);
 }
 
 constexpr int ADMIT_THREADS = 256;
@@ -413,22 +414,49 @@ extern "C" int tn_attn_decode_bf16(const void* Q, int64_t ldq, const void* K, co
   return TN_OK;
 }
 
+// the checks of both K/V copies (`map`: row_end or the admission table): pointers, dims, strides, 16-byte alignment
+static int check_kv_copy(const char* fn, const void* K, int64_t ldk, const void* V, int64_t ldv, const void* Kc,
+                         const void* Vc, int64_t ld_tok, int64_t ld_batch, const void* map, int B, int S_cap,
+                         int width) {
+  TN_REQUIRE(K && V && Kc && Vc && map, "%s: null pointer", fn);
+  TN_REQUIRE(B > 0 && S_cap > 0 && width > 0 && width % 8 == 0, "%s: bad dims B=%d S_cap=%d width=%d", fn, B, S_cap,
+             width);
+  TN_REQUIRE(ldk % 8 == 0 && ldv % 8 == 0 && ld_tok % 8 == 0 && ld_batch % 8 == 0 && ldk >= width && ldv >= width &&
+                 ld_tok >= width && ld_batch >= ld_tok * S_cap, "%s: bad strides", fn);
+  TN_REQUIRE(((uintptr_t(K) | uintptr_t(V) | uintptr_t(Kc) | uintptr_t(Vc)) & 15) == 0,
+             "%s: pointers must be 16-byte aligned", fn);
+  return TN_OK;
+}
+
 extern "C" int tn_kv_append_bf16(const void* K, int64_t ldk, const void* V, int64_t ldv, void* K_cache, void* V_cache,
                                  int64_t ld_tok, int64_t ld_batch, const int32_t* row_end, int B, int T_new, int S_cap,
                                  int width, tn_stream_t stream_) {
   clear_error();
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  TN_REQUIRE(K && V && K_cache && V_cache && row_end, "tn_kv_append_bf16: null pointer");
-  TN_REQUIRE(B > 0 && T_new > 0 && S_cap >= T_new && width > 0 && width % 8 == 0,
-             "tn_kv_append_bf16: bad dims B=%d T_new=%d S_cap=%d width=%d", B, T_new, S_cap, width);
-  TN_REQUIRE(ldk % 8 == 0 && ldv % 8 == 0 && ld_tok % 8 == 0 && ld_batch % 8 == 0 && ldk >= width && ldv >= width &&
-                 ld_tok >= width && ld_batch >= ld_tok * S_cap, "tn_kv_append_bf16: bad strides");
+  if (const int rc = check_kv_copy("tn_kv_append_bf16", K, ldk, V, ldv, K_cache, V_cache, ld_tok, ld_batch, row_end,
+                                   B, S_cap, width)) return rc;
+  TN_REQUIRE(T_new > 0 && S_cap >= T_new, "tn_kv_append_bf16: bad dims T_new=%d S_cap=%d", T_new, S_cap);
   TN_REQUIRE(T_new <= 65535 && B <= 65535, "tn_kv_append_bf16: grid too large");
-  TN_REQUIRE(((uintptr_t(K) | uintptr_t(V) | uintptr_t(K_cache) | uintptr_t(V_cache)) & 15) == 0,
-             "tn_kv_append_bf16: pointers must be 16-byte aligned");
   kv_append_kernel<<<dim3(T_new, B), 128, 0, stream>>>(
       static_cast<const bf16*>(K), ldk, static_cast<const bf16*>(V), ldv, static_cast<bf16*>(K_cache),
       static_cast<bf16*>(V_cache), ld_tok, ld_batch, row_end, T_new, S_cap, width);
+  TN_CHECK_CUDA(cudaGetLastError());
+  return TN_OK;
+}
+
+// both selection launches, one CTA per logits row: processor arguments, bitmap bytes, one-time shared-memory opt-in
+template <auto kernel, typename... Args>
+static int select_launch(const char* fn, int rows, int V, float penalty, int ngram, tn_stream_t stream, Args... args) {
+  TN_REQUIRE(penalty > 0.f, "%s: repetition_penalty must be > 0", fn);
+  TN_REQUIRE(ngram >= 0, "%s: no_repeat_ngram_size must be >= 0", fn);
+  const size_t smem = size_t(2) * ((V + 31) / 32) * sizeof(uint32_t);
+  TN_REQUIRE(smem <= SEL_MAX_SMEM, "%s: vocabulary of %d too large for the shared-memory bitmaps", fn, V);
+  static bool configured = false;
+  if (!configured) {
+    TN_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SEL_MAX_SMEM));
+    configured = true;
+  }
+  kernel<<<rows, SEL_THREADS, smem, static_cast<cudaStream_t>(stream)>>>(args...);
   TN_CHECK_CUDA(cudaGetLastError());
   return TN_OK;
 }
@@ -438,23 +466,11 @@ extern "C" int tn_greedy_select_bf16(const void* logits, int64_t ld, int B, int 
                                      float repetition_penalty, int no_repeat_ngram_size, int64_t eos, int64_t pad,
                                      tn_stream_t stream_) {
   clear_error();
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   TN_REQUIRE(logits && history && length && positions && next_ids && finished, "tn_greedy_select_bf16: null pointer");
   TN_REQUIRE(B > 0 && V > 0 && ld >= V && ld_hist > 0, "tn_greedy_select_bf16: bad dims B=%d V=%d", B, V);
-  TN_REQUIRE(repetition_penalty > 0.f, "tn_greedy_select_bf16: repetition_penalty must be > 0");
-  TN_REQUIRE(no_repeat_ngram_size >= 0, "tn_greedy_select_bf16: no_repeat_ngram_size must be >= 0");
-  const size_t smem = size_t(2) * ((V + 31) / 32) * sizeof(uint32_t);
-  TN_REQUIRE(smem <= 200 * 1024, "tn_greedy_select_bf16: vocabulary of %d too large for the shared-memory bitmaps", V);
-  static bool configured = false;
-  if (!configured) {
-    TN_CHECK_CUDA(cudaFuncSetAttribute(greedy_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    configured = true;
-  }
-  greedy_select_kernel<<<B, SEL_THREADS, smem, stream>>>(static_cast<const bf16*>(logits), ld, V, history, ld_hist,
-                                                         length, positions, next_ids, finished, repetition_penalty,
-                                                         no_repeat_ngram_size, eos, pad);
-  TN_CHECK_CUDA(cudaGetLastError());
-  return TN_OK;
+  return select_launch<greedy_select_kernel>(
+      "tn_greedy_select_bf16", B, V, repetition_penalty, no_repeat_ngram_size, stream_, static_cast<const bf16*>(logits),
+      ld, V, history, ld_hist, length, positions, next_ids, finished, repetition_penalty, no_repeat_ngram_size, eos, pad);
 }
 
 extern "C" int tn_greedy_select_slots_bf16(const void* logits, int64_t ld, int n_rows, const int32_t* row_slot, int B,
@@ -463,7 +479,6 @@ extern "C" int tn_greedy_select_slots_bf16(const void* logits, int64_t ld, int n
                                            float repetition_penalty, int no_repeat_ngram_size, int64_t eos, int64_t pad,
                                            tn_stream_t stream_) {
   clear_error();
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   TN_REQUIRE(logits && history && length && positions && next_ids && finished && limit,
              "tn_greedy_select_slots_bf16: null pointer");
   TN_REQUIRE(n_rows > 0 && B > 0 && V > 0 && ld >= V && ld_hist > 0, "tn_greedy_select_slots_bf16: bad dims n_rows=%d "
@@ -472,11 +487,6 @@ extern "C" int tn_greedy_select_slots_bf16(const void* logits, int64_t ld, int n
              "must equal B (%d)", n_rows, B);
   TN_REQUIRE(!row_slot || n_rows <= SEL_MAX_MAP, "tn_greedy_select_slots_bf16: at most %d mapped rows, got %d",
              SEL_MAX_MAP, n_rows);
-  TN_REQUIRE(repetition_penalty > 0.f, "tn_greedy_select_slots_bf16: repetition_penalty must be > 0");
-  TN_REQUIRE(no_repeat_ngram_size >= 0, "tn_greedy_select_slots_bf16: no_repeat_ngram_size must be >= 0");
-  const size_t smem = size_t(2) * ((V + 31) / 32) * sizeof(uint32_t);
-  TN_REQUIRE(smem <= 200 * 1024, "tn_greedy_select_slots_bf16: vocabulary of %d too large for the shared-memory bitmaps",
-             V);
   SlotMap map{};
   map.use_map = row_slot != nullptr;
   for (int r = 0; row_slot && r < n_rows; ++r) {   // the map is host memory: checked here, passed by value
@@ -486,17 +496,10 @@ extern "C" int tn_greedy_select_slots_bf16(const void* logits, int64_t ld, int n
       TN_REQUIRE(row_slot[q] != row_slot[r], "tn_greedy_select_slots_bf16: slot %d named twice", row_slot[r]);
     map.slot[r] = row_slot[r];
   }
-  static bool configured = false;
-  if (!configured) {
-    TN_CHECK_CUDA(cudaFuncSetAttribute(greedy_select_slots_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       200 * 1024));
-    configured = true;
-  }
-  greedy_select_slots_kernel<<<n_rows, SEL_THREADS, smem, stream>>>(
+  return select_launch<greedy_select_slots_kernel>(
+      "tn_greedy_select_slots_bf16", n_rows, V, repetition_penalty, no_repeat_ngram_size, stream_,
       static_cast<const bf16*>(logits), ld, V, history, ld_hist, length, positions, next_ids, finished, limit,
       repetition_penalty, no_repeat_ngram_size, eos, pad, map);
-  TN_CHECK_CUDA(cudaGetLastError());
-  return TN_OK;
 }
 
 // docs: host [n_docs][4] int32 = (src_row, slot, len, limit); checked against the cache shape, returned by value
@@ -524,13 +527,9 @@ extern "C" int tn_kv_scatter_bf16(const void* K, int64_t ldk, const void* V, int
                                   int n_docs, int B, int S_cap, int width, tn_stream_t stream_) {
   clear_error();
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  TN_REQUIRE(K && V && K_cache && V_cache && docs, "tn_kv_scatter_bf16: null pointer");
-  TN_REQUIRE(B > 0 && S_cap > 0 && width > 0 && width % 8 == 0 && n_src_rows > 0,
-             "tn_kv_scatter_bf16: bad dims B=%d S_cap=%d width=%d", B, S_cap, width);
-  TN_REQUIRE(ldk % 8 == 0 && ldv % 8 == 0 && ld_tok % 8 == 0 && ld_batch % 8 == 0 && ldk >= width && ldv >= width &&
-                 ld_tok >= width && ld_batch >= ld_tok * S_cap, "tn_kv_scatter_bf16: bad strides");
-  TN_REQUIRE(((uintptr_t(K) | uintptr_t(V) | uintptr_t(K_cache) | uintptr_t(V_cache)) & 15) == 0,
-             "tn_kv_scatter_bf16: pointers must be 16-byte aligned");
+  if (const int rc = check_kv_copy("tn_kv_scatter_bf16", K, ldk, V, ldv, K_cache, V_cache, ld_tok, ld_batch, docs,
+                                   B, S_cap, width)) return rc;
+  TN_REQUIRE(n_src_rows > 0, "tn_kv_scatter_bf16: bad dims: %lld source rows", (long long)n_src_rows);
   AdmitTable tab{};
   int max_len = 0;
   const int rc = admit_table("tn_kv_scatter_bf16", docs, n_docs, B, S_cap, n_src_rows, &tab, &max_len);

@@ -58,6 +58,7 @@ class B200KVCache:
         dev = torch.device(device) if device is not None else lm.lm_head.weight.device
         self.B, self.S_cap = int(batch_size), int(max_length)
         self.L, self.H, self.KV, self.hd = len(lm.model.layers), a.num_heads, a.num_key_value_heads, a.head_dim
+        self.scale = 1.0 / math.sqrt(self.hd)       # softmax scale of the attention
         if self.B <= 0 or self.S_cap <= 0:
             raise TouchNetB200Error(f"B200KVCache: batch_size {batch_size} / max_length {max_length} must be positive")
         self.vocab = cfg.vocab_size
@@ -154,8 +155,16 @@ def _logits_last(w: _Weights, x_last: torch.Tensor) -> torch.Tensor:
     return ops.gemm(h, w.lm_head)
 
 
-def _prompt_embeds(model, input_ids, input_features, w: _Weights):
-    lm, audio = _parts(model)
+def _default_positions(attention_mask: torch.Tensor) -> torch.Tensor:
+    """hf GenerationMixin: cumsum of the mask, 1 at padding."""
+    m = (attention_mask != 0).to(torch.int64)
+    return (m.cumsum(-1) - 1).masked_fill_(m == 0, 1)
+
+
+def _prompt_front(model, w: _Weights, input_ids, input_features, doc, pos):
+    """Embeddings of the prompt [B, T] (their NaN flag raised here), the AttnPlan of its document ids `doc` and the rope
+    tables of its positions `pos`: (x, plan, cos, sin)."""
+    _, audio = _parts(model)
     B, T = input_ids.shape
     d = w.embed.shape[1]
     proj, nan_flag = None, None
@@ -167,6 +176,16 @@ def _prompt_embeds(model, input_ids, input_features, w: _Weights):
     x = ops.embed_add(input_ids.reshape(-1).contiguous(), w.embed, proj, B * T, d, nan_flag)
     if audio is not None:
         audio.raise_if_nan()
+    return (x, ops.AttnPlan(doc), *ops.rope_table(pos, w.inv_freq, w.rope_scaling))
+
+
+def _layers(cache: B200KVCache, w: _Weights, x, cos, sin, attend):
+    """Every block over the rows x; `attend(q, k, v, k_cache, v_cache) -> (o, lse)` stores the layer's K/V into its
+    cache and runs the attention."""
+    for i, lw in enumerate(w.layers):
+        kc, vc = cache.layer(i)
+        x, _ = ops.block_forward(x, *lw, cos, sin, cache.H, cache.KV, w.eps, cache.hd,
+                                 lambda q, k, v, kc=kc, vc=vc: (*attend(q, k, v, kc, vc), k, v), need_gu=False)
     return x
 
 
@@ -183,29 +202,19 @@ def prefill(model, cache: B200KVCache, input_ids, input_features=None, attention
     if attention_mask is None:
         attention_mask = torch.ones((B, T), dtype=torch.int64, device=dev)
     _check_mask(attention_mask, B, T)
-    if position_ids is None:          # hf GenerationMixin: cumsum of the mask, 1 at padding
-        m = (attention_mask != 0).to(torch.int64)
-        position_ids = (m.cumsum(-1) - 1).masked_fill_(m == 0, 1)
-    position_ids = position_ids.to(torch.int64)
-    x = _prompt_embeds(model, input_ids, input_features, w)
-    plan = ops.AttnPlan(attention_mask)
-    cos, sin = ops.rope_table(position_ids, w.inv_freq, w.rope_scaling)
+    position_ids = (_default_positions(attention_mask) if position_ids is None else position_ids).to(torch.int64)
+    x, plan, cos, sin = _prompt_front(model, w, input_ids, input_features, attention_mask, position_ids)
     cache.kv_start.copy_(_last_doc_start(attention_mask))
-    cache.kv_end.fill_(T)
+    cache.kv_end.fill_(T)          # read by kv_append: the state is written before the layers run
     cache.positions.copy_(position_ids[:, -1])
     cache.history[:, :T] = input_ids
     cache.finished.zero_()
-    H, KV, hd = cache.H, cache.KV, cache.hd
-    scale = 1.0 / math.sqrt(hd)
-    for i, lw in enumerate(w.layers):
-        kc, vc = cache.layer(i)
 
-        def attend(q, k, v, kc=kc, vc=vc):
-            ops.kv_append(k, v, kc, vc, cache.kv_end, T)
-            o, lse = ops.attn_fwd(q, k, v, plan, H, KV, scale)
-            return o, lse, k, v
+    def attend(q, k, v, kc, vc):
+        ops.kv_append(k, v, kc, vc, cache.kv_end, T)
+        return ops.attn_fwd(q, k, v, plan, cache.H, cache.KV, cache.scale)
 
-        x, _ = ops.block_forward(x, *lw, cos, sin, H, KV, w.eps, hd, attend, need_gu=False)
+    x = _layers(cache, w, x, cos, sin, attend)
     cache.length = T
     return _logits_last(w, x.view(B, T, -1)[:, -1].contiguous())
 
@@ -218,18 +227,13 @@ def decode_step(model, cache: B200KVCache, weights: Optional[_Weights] = None) -
     B = cache.B
     x = ops.embed_add(cache.next_ids, w.embed, None, B, w.embed.shape[1], None if audio is None else audio._nan_flag)
     cos, sin = ops.rope_table(cache.positions, w.inv_freq, w.rope_scaling)
-    H, KV, hd = cache.H, cache.KV, cache.hd
-    scale = 1.0 / math.sqrt(hd)
-    for i, lw in enumerate(w.layers):
-        kc, vc = cache.layer(i)
 
-        def attend(q, k, v, kc=kc, vc=vc):
-            ops.kv_append(k, v, kc, vc, cache.kv_end, 1)
-            o = ops.attn_decode(q, kc, vc, cache.kv_start, cache.kv_end, H, KV, scale, cache.workspace)
-            return o, None, k, v
+    def attend(q, k, v, kc, vc):
+        ops.kv_append(k, v, kc, vc, cache.kv_end, 1)
+        o = ops.attn_decode(q, kc, vc, cache.kv_start, cache.kv_end, cache.H, cache.KV, cache.scale, cache.workspace)
+        return o, None
 
-        x, _ = ops.block_forward(x, *lw, cos, sin, H, KV, w.eps, hd, attend, need_gu=False)
-    return _logits_last(w, x)
+    return _logits_last(w, _layers(cache, w, x, cos, sin, attend))
 
 
 def forward_cached(model, cache: B200KVCache, input_ids, input_features=None, attention_mask=None, position_ids=None):
@@ -279,6 +283,37 @@ def _validate(max_new_tokens, eos_token_id, pad_token_id, repetition_penalty, no
         raise TouchNetB200Error(f"generate: unsupported arguments {bad}")
 
 
+def _captured(step, capture: bool):
+    """`step` (no arguments, device state only) as a callable that runs it eagerly the first time, then, if `capture`,
+    captures it once in a CUDA graph and replays the graph; without `capture` every call runs eagerly."""
+    graph, calls = None, 0
+
+    def run():
+        nonlocal graph, calls
+        if graph is None and calls >= 1 and capture:
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph):
+                step()
+        if graph is not None:
+            graph.replay()
+        else:
+            step()
+        calls += 1
+
+    return run
+
+
+def _host_sync(flags, nan_flag) -> list:
+    """The one host sync per decode step: the int32 tensors `flags` and the NaN flag read in one `.tolist()`.  A set NaN
+    flag is zeroed and raises ValueError; otherwise returns the values of `flags`, flattened."""
+    flags = [f.reshape(-1) for f in flags] + ([] if nan_flag is None else [nan_flag])
+    vals = (flags[0] if len(flags) == 1 else torch.cat(flags)).tolist()
+    if nan_flag is not None and vals.pop() != 0:
+        nan_flag.zero_()
+        raise ValueError("NaN in data.")
+    return vals
+
+
 def generate(model, input_ids, input_features=None, attention_mask=None, position_ids=None, *, max_new_tokens,
              eos_token_id, pad_token_id, repetition_penalty=1.0, no_repeat_ngram_size=0, do_sample=False, num_beams=1,
              use_cache=True, bos_token_id=None, top_k=None, top_p=None, temperature=None, early_stopping=None, **kwargs):
@@ -302,31 +337,14 @@ def generate(model, input_ids, input_features=None, attention_mask=None, positio
             ops.greedy_select(logits, cache.history, cache.kv_end, cache.positions, cache.next_ids, cache.finished,
                               float(repetition_penalty), int(no_repeat_ngram_size), eos, pad)
 
-        def done() -> bool:   # the one host sync per step
-            flags = cache.finished.min().reshape(1)
-            if nan_flag is not None:
-                flags = torch.cat([flags, nan_flag.reshape(1).to(flags.dtype)])
-            vals = flags.tolist()
-            if len(vals) > 1 and vals[1] != 0:
-                nan_flag.zero_()
-                raise ValueError("NaN in data.")
-            return vals[0] != 0
-
         select(prefill(model, cache, input_ids, input_features, attention_mask, position_ids, weights=w))
+        step = _captured(lambda: select(decode_step(model, cache, weights=w)), input_ids.is_cuda)
         n = 1
-        graph = None
-        while n < max_new and not done():
-            if graph is None and n >= 2 and input_ids.is_cuda:
-                graph = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(graph):
-                    select(decode_step(model, cache, weights=w))
-            if graph is not None:
-                graph.replay()
-            else:
-                select(decode_step(model, cache, weights=w))     # the first decode step runs eagerly
+        while n < max_new and not _host_sync([cache.finished.min()], nan_flag)[0]:
+            step()
             n += 1
         if n == max_new and nan_flag is not None:
-            done()
+            _host_sync([], nan_flag)
     return cache.history[:, :T + n].clone()
 
 
@@ -364,9 +382,8 @@ class _Prompt:
         mask = torch.ones(T, dtype=torch.int64, device=dev) if mask is None else mask.to(dev, torch.int64)
         _check_mask(mask.reshape(1, -1), 1, T)
         pos = p.get("position_ids")
-        if pos is None:                   # as prefill: cumsum of the mask, 1 at padding
-            m = (mask != 0).to(torch.int64)
-            pos = (m.cumsum(-1) - 1).masked_fill_(m == 0, 1)
+        if pos is None:
+            pos = _default_positions(mask)
         elif tuple(pos.shape) != (T,):
             raise TouchNetB200Error(f"generate_many: prompt {index}: position_ids must be [{T}]")
         self.index, self.T, self.budget = index, T, budget
@@ -410,22 +427,16 @@ def _admit(model, cache: B200KVCache, limit: torch.Tensor, w: _Weights, batch, p
         if feats is not None and p.feats is not None and p.T != 1:     # as generate: no projector on a 1-token prompt
             feats[o0:o0 + p.T] = p.feats.to(BF16)
         docs.append((o0, slot, p.T, p.T + p.budget))
-    x = _prompt_embeds(model, ids.view(1, n), None if feats is None else feats.view(1, n, -1), w)
-    plan = ops.AttnPlan(doc.view(1, n))
-    cos, sin = ops.rope_table(pos.view(1, n), w.inv_freq, w.rope_scaling)
+    x, plan, cos, sin = _prompt_front(model, w, ids.view(1, n), None if feats is None else feats.view(1, n, -1),
+                                      doc.view(1, n), pos.view(1, n))
     ops.slot_admit(docs, ids, plan.doc.view(-1), pos, cache.history, cache.kv_start, cache.kv_end, cache.positions,
                    cache.finished, limit)
-    H, KV, hd = cache.H, cache.KV, cache.hd
-    scale = 1.0 / math.sqrt(hd)
-    for i, lw in enumerate(w.layers):
-        kc, vc = cache.layer(i)
 
-        def attend(q, k, v, kc=kc, vc=vc):
-            ops.kv_scatter(k, v, kc, vc, docs)
-            o, lse = ops.attn_fwd(q, k, v, plan, H, KV, scale)
-            return o, lse, k, v
+    def attend(q, k, v, kc, vc):
+        ops.kv_scatter(k, v, kc, vc, docs)
+        return ops.attn_fwd(q, k, v, plan, cache.H, cache.KV, cache.scale)
 
-        x, _ = ops.block_forward(x, *lw, cos, sin, H, KV, w.eps, hd, attend, need_gu=False)
+    x = _layers(cache, w, x, cos, sin, attend)
     last = torch.tensor([o0 + p.T - 1 for (_, p), o0 in zip(batch, offs)], dtype=torch.int64).to(dev)
     select(_logits_last(w, x.index_select(0, last)), [slot for slot, _ in batch])
 
@@ -491,12 +502,7 @@ def generate_many(model, prompts, *, batch_size, max_new_tokens, eos_token_id, p
         admission_events = []
         admissions = 0
 
-        def select_decode(logits):
-            ops.greedy_select_slots(logits, cache.history, cache.kv_end, cache.positions, cache.next_ids,
-                                    cache.finished, limit, float(repetition_penalty), int(no_repeat_ngram_size), eos,
-                                    pad)
-
-        def select_admitted(logits, slots):
+        def select(logits, slots=None):
             ops.greedy_select_slots(logits, cache.history, cache.kv_end, cache.positions, cache.next_ids,
                                     cache.finished, limit, float(repetition_penalty), int(no_repeat_ngram_size), eos,
                                     pad, row_slot=slots)
@@ -520,7 +526,7 @@ def generate_many(model, prompts, *, batch_size, max_new_tokens, eos_token_id, p
                 if stats is not None and dev.type == "cuda":
                     ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
                     ev[0].record()
-                _admit(model, cache, limit, w, chunk, pad, select_admitted)
+                _admit(model, cache, limit, w, chunk, pad, select)
                 admissions += 1
                 if ev is not None:
                     ev[1].record()
@@ -528,26 +534,13 @@ def generate_many(model, prompts, *, batch_size, max_new_tokens, eos_token_id, p
                 for slot, p in chunk:
                     slot_prompt[slot] = p
 
-        def step() -> None:
-            select_decode(decode_step(model, cache, weights=w))
-
+        step = _captured(lambda: select(decode_step(model, cache, weights=w)), cuda_graph and dev.type == "cuda")
         admit(list(range(B)))
-        graph, steps = None, 0
+        steps = 0
         while any(p is not None for p in slot_prompt):
-            if graph is None and steps >= 1 and cuda_graph and dev.type == "cuda":
-                graph = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(graph):
-                    step()
-            if graph is not None:
-                graph.replay()
-            else:
-                step()                        # the first decode step runs eagerly
+            step()
             steps += 1
-            flags = torch.cat([cache.finished, cache.kv_end] + ([] if nan_flag is None else [nan_flag.reshape(1)]))
-            vals = flags.tolist()             # the one host sync per step
-            if nan_flag is not None and vals[-1] != 0:
-                nan_flag.zero_()
-                raise ValueError("NaN in data.")
+            vals = _host_sync([cache.finished, cache.kv_end], nan_flag)
             free = []
             for s in range(B):
                 p = slot_prompt[s]

@@ -397,25 +397,38 @@ def attn_decode(q, k_cache, v_cache, kv_start, kv_end, H: int, KV: int, scale: f
     return (o, lse_t) if lse else o
 
 
-def kv_append(k, v, k_cache, v_cache, row_end, T_new: int):
-    """Cache rows [row_end[b] - T_new, row_end[b]) of batch row b <- rows b*T_new .. of k / v [B*T_new, KV*128]."""
-    _chk(k, "k", BF16); _chk(v, "v", BF16); _chk(k_cache, "k_cache", BF16); _chk(row_end, "row_end", torch.int32)
+def _kv_copy_dims(k, v, k_cache, v_cache):
+    """The checks both K/V copies make; returns the cache's (B, S_cap, width)."""
+    _chk(k, "k", BF16); _chk(v, "v", BF16); _chk(k_cache, "k_cache", BF16)
     B, S_cap, width = k_cache.shape
     assert k_cache.stride() == v_cache.stride() and k.shape[1] == width and k.stride(1) == 1 and v.stride(1) == 1
+    return B, S_cap, width
+
+
+def kv_append(k, v, k_cache, v_cache, row_end, T_new: int):
+    """Cache rows [row_end[b] - T_new, row_end[b]) of batch row b <- rows b*T_new .. of k / v [B*T_new, KV*128]."""
+    B, S_cap, width = _kv_copy_dims(k, v, k_cache, v_cache)
+    _chk(row_end, "row_end", torch.int32)
     _lib.call("tn_kv_append_bf16", k.data_ptr(), k.stride(0), v.data_ptr(), v.stride(0), k_cache.data_ptr(),
               v_cache.data_ptr(), k_cache.stride(1), k_cache.stride(0), row_end.data_ptr(), B, int(T_new), S_cap, width,
               _st())
+
+
+def _select_dims(logits, history, length, positions, next_ids, finished):
+    """The checks both selections make of the logits and the decoding state; returns the logits' (rows, V)."""
+    _chk(logits, "logits", BF16); _chk(history, "history", torch.int64); _chk(length, "length", torch.int32)
+    _chk(positions, "positions", torch.int64); _chk(next_ids, "next_ids", torch.int64)
+    _chk(finished, "finished", torch.int32)
+    assert logits.stride(1) == 1 and history.stride(1) == 1
+    return logits.shape
 
 
 def greedy_select(logits, history, length, positions, next_ids, finished, repetition_penalty: float,
                   no_repeat_ngram_size: int, eos: int, pad: int):
     """Greedy next token of every row (HF repetition penalty + no-repeat-ngram + argmax on fp32-cast bf16 logits [B, V]),
     written into history / next_ids; advances length and positions, updates finished (all device tensors, in place)."""
-    _chk(logits, "logits", BF16); _chk(history, "history", torch.int64); _chk(length, "length", torch.int32)
-    _chk(positions, "positions", torch.int64); _chk(next_ids, "next_ids", torch.int64)
-    _chk(finished, "finished", torch.int32)
-    B, V = logits.shape
-    assert logits.stride(1) == 1 and history.stride(1) == 1 and history.shape[0] == B
+    B, V = _select_dims(logits, history, length, positions, next_ids, finished)
+    assert history.shape[0] == B
     _lib.call("tn_greedy_select_bf16", logits.data_ptr(), logits.stride(0), B, V, history.data_ptr(), history.stride(0),
               length.data_ptr(), positions.data_ptr(), next_ids.data_ptr(), finished.data_ptr(),
               float(repetition_penalty), int(no_repeat_ngram_size), int(eos), int(pad), _st())
@@ -429,9 +442,7 @@ def _host_i32(rows) -> torch.Tensor:
 def kv_scatter(k, v, k_cache, v_cache, docs):
     """Cache rows [0, len) of slot `slot` <- rows [src_row, src_row + len) of k / v [rows, KV*128], for each
     (src_row, slot, len, limit) in `docs` (a list; limit is not used here)."""
-    _chk(k, "k", BF16); _chk(v, "v", BF16); _chk(k_cache, "k_cache", BF16)
-    B, S_cap, width = k_cache.shape
-    assert k_cache.stride() == v_cache.stride() and k.shape[1] == width and k.stride(1) == 1 and v.stride(1) == 1
+    B, S_cap, width = _kv_copy_dims(k, v, k_cache, v_cache)
     tab = _host_i32(docs)
     _lib.call("tn_kv_scatter_bf16", k.data_ptr(), k.stride(0), v.data_ptr(), v.stride(0), k.shape[0], k_cache.data_ptr(),
               v_cache.data_ptr(), k_cache.stride(1), k_cache.stride(0), tab.data_ptr(), len(docs), B, S_cap, width, _st())
@@ -453,11 +464,8 @@ def greedy_select_slots(logits, history, length, positions, next_ids, finished, 
                         no_repeat_ngram_size: int, eos: int, pad: int, row_slot=None):
     """greedy_select over cache slots: logits row r selects for slot row_slot[r] (a list; None = slot r).  Finished or
     idle slots do not advance (pad in next_ids); a slot finishes on eos or when its length reaches limit."""
-    _chk(logits, "logits", BF16); _chk(history, "history", torch.int64); _chk(length, "length", torch.int32)
-    _chk(positions, "positions", torch.int64); _chk(next_ids, "next_ids", torch.int64)
-    _chk(finished, "finished", torch.int32); _chk(limit, "limit", torch.int32)
-    n, V = logits.shape
-    assert logits.stride(1) == 1 and history.stride(1) == 1
+    n, V = _select_dims(logits, history, length, positions, next_ids, finished)
+    _chk(limit, "limit", torch.int32)
     tab = None if row_slot is None else _host_i32(row_slot)
     _lib.call("tn_greedy_select_slots_bf16", logits.data_ptr(), logits.stride(0), n, None if tab is None else tab.data_ptr(),
               history.shape[0], V, history.data_ptr(), history.stride(0), length.data_ptr(), positions.data_ptr(),
