@@ -168,6 +168,31 @@ int tn_greedy_select_bf16(const void* logits, int64_t ld, int B, int V, int64_t*
                           float repetition_penalty, int no_repeat_ngram_size, int64_t eos, int64_t pad,
                           tn_stream_t stream);
 
+/* Speculative decoding (generation.generate with assistant_model): a draft model proposes k tokens per row, the target
+ * scores the k + 1 rows next_ids, d_0 .. d_{k-1} in one step and keeps the longest prefix that matches its own picks.
+ *   tn_attn_decode_multi: Tq query rows per batch row, Q [B*Tq, H*128]: row b*Tq + j is query j of batch row b, at cache
+ *     position kv_end[b] - Tq + j, attending to cache rows [kv_start[b], kv_end[b] - Tq + j + 1) (causal within the new
+ *     block).  Row j's O / lse are bit-identical to tn_attn_decode_bf16 with kv_end = kv_end[b] - Tq + j + 1: same
+ *     split count and chunks (functions of B, KV, S_cap), same merge order.  `workspace` holds
+ *     tn_attn_decode_multi_ws_floats(B, Tq, H, KV, S_cap) floats.  Tq * H/KV in 1..16 (one m16 tile per kv head).
+ *   tn_verify_select: logits [B*(k+1), V] (row b*(k+1) + j), draft [B, k] int64 (device).  For a row with finished == 0,
+ *     picks[b, j] is the pick of tn_greedy_select on logits row b*(k+1) + j over history[b, 0:length[b]] followed by
+ *     draft[b, 0:j]; n = the number of leading j < k with draft[b, j] == picks[b, j].  The row emits picks[b, 0..n],
+ *     cut after the first eos and when length reaches limit[b]: they are written to history[b, length[b]..],
+ *     length and positions advance by their count, next_ids = the last one, finished = 1 if it is eos or length ==
+ *     limit[b].  A finished row does not advance (next_ids = pad, nothing else written).  picks [B, k+1] int64 is
+ *     written for every row that is not finished.
+ */
+int64_t tn_attn_decode_multi_ws_floats(int B, int Tq, int H, int KV, int S_cap);
+int tn_attn_decode_multi_bf16(const void* Q, int64_t ldq, const void* K, const void* V, int64_t ld_tok,
+                              int64_t ld_batch, const int32_t* kv_start, const int32_t* kv_end, int B, int Tq, int H,
+                              int KV, int S_cap, float scale, float* workspace, void* O, int64_t ldo, float* lse,
+                              tn_stream_t stream);
+int tn_verify_select_bf16(const void* logits, int64_t ld, int B, int k, int V, const int64_t* draft, int64_t* history,
+                          int64_t ld_hist, int32_t* length, int64_t* positions, int64_t* next_ids, int32_t* finished,
+                          const int32_t* limit, int64_t* picks, float repetition_penalty, int no_repeat_ngram_size,
+                          int64_t eos, int64_t pad, tn_stream_t stream);
+
 /* Continuous batching (generation.generate_many): a cache of B slots whose rows are refilled with new prompts while
  * the other slots keep decoding.  `docs` is a HOST table [n_docs][4] int32 = (src_row, slot, len, limit), at most
  * TN_ADMIT_MAX documents per call, distinct slots in [0, B), 0 < len < limit <= S_cap; it is checked here and passed to

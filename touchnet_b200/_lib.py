@@ -42,8 +42,13 @@ _SIGNATURES = {
                          _vp, _i64, _vp, _vp, _i, _i, _i, _i, _f, _i, _i, _vp, _vp, _vp, _vp, _vp],
     "tn_attn_decode_ws_floats": [_i, _i, _i, _i],
     "tn_attn_decode_bf16": [_vp, _i64, _vp, _vp, _i64, _i64, _vp, _vp, _i, _i, _i, _i, _f, _vp, _vp, _i64, _vp, _vp],
+    "tn_attn_decode_multi_ws_floats": [_i, _i, _i, _i, _i],
+    "tn_attn_decode_multi_bf16": [_vp, _i64, _vp, _vp, _i64, _i64, _vp, _vp, _i, _i, _i, _i, _i, _f, _vp, _vp, _i64, _vp,
+                                  _vp],
     "tn_kv_append_bf16": [_vp, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _vp, _i, _i, _i, _i, _vp],
     "tn_greedy_select_bf16": [_vp, _i64, _i, _i, _vp, _i64, _vp, _vp, _vp, _vp, _f, _i, _i64, _i64, _vp],
+    "tn_verify_select_bf16": [_vp, _i64, _i, _i, _i, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _f, _i, _i64, _i64,
+                              _vp],
     "tn_greedy_select_slots_bf16": [_vp, _i64, _i, _vp, _i, _i, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _f, _i, _i64, _i64,
                                     _vp],
     "tn_kv_scatter_bf16": [_vp, _i64, _vp, _i64, _i64, _vp, _vp, _i64, _i64, _vp, _i, _i, _i, _i, _vp],
@@ -72,7 +77,8 @@ _SIGNATURES = {
     "tn_pack_ce_fused_bf16": [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _f, _i64, _i, _vp],
     "tn_adamw_f32": [_vp, _vp, _vp, _vp, _vp, _i64, _f, _f, _f, _f, _f, _f, _f, _vp, _vp],
 }
-_RESTYPES = {"tn_last_error": c_char_p, "tn_attn_meta_ints": c_int64, "tn_attn_decode_ws_floats": c_int64}
+_RESTYPES = {"tn_last_error": c_char_p, "tn_attn_meta_ints": c_int64, "tn_attn_decode_ws_floats": c_int64,
+             "tn_attn_decode_multi_ws_floats": c_int64}
 
 EXPORTED_SYMBOLS = sorted(list(_SIGNATURES) + ["tn_last_error"])
 
@@ -106,7 +112,8 @@ def load(path: str | None = None) -> ctypes.CDLL:
 
 
 # kernels launched per entry point (for bench.py's `gpu_launches` claim)
-_LAUNCHES = {"tn_attn_prep": 3, "tn_attn_bwd_bf16": 3, "tn_attn_decode_bf16": 2, "tn_logmel_power_f32": 2,
+_LAUNCHES = {"tn_attn_prep": 3, "tn_attn_bwd_bf16": 3, "tn_attn_decode_bf16": 2, "tn_attn_decode_multi_bf16": 2,
+             "tn_verify_select_bf16": 2, "tn_logmel_power_f32": 2,
              "tn_rmsnorm_bwd_bf16": 2, "tn_pack_layout_i64": 2}
 launch_count = 0
 _hooks = []   # callables(name, phase) with phase in {"pre", "post"}; bench.py uses them to time kernel classes

@@ -14,6 +14,11 @@
 // Continuous batching (generation.generate_many) adds slot-addressed forms: a K/V scatter of a packed multi-prompt
 // prefill into chosen cache slots, the admission of those slots' decoding state, and a selection that holds finished /
 // idle slots still and stops a slot at its token limit.
+//
+// Speculative decoding (generation.generate with assistant_model) adds the multi-query form of the decode attention
+// (Tq new rows per sequence, causal within the block, each row bit-identical to the single-query kernel at its own
+// length) and a verify selection: the greedy pick at each of the k + 1 positions of the block over the history
+// extended by the draft tokens before it, then the longest accepted prefix plus one token.
 #include "../../include/touchnet_b200.h"
 #include "attn_common.cuh"
 #include "host.h"
@@ -45,12 +50,18 @@ struct DecodeParams {
   int64_t ldq, ld_tok, ld_batch;
   const int32_t* kv_start;
   const int32_t* kv_end;
-  float* part_o;    // [B, H, splits, 128]
-  float* part_ml;   // [B, H, splits, 2]  (m in the log2 domain, l)
+  float* part_o;    // [B*Tq, H, splits, 128]
+  float* part_ml;   // [B*Tq, H, splits, 2]  (m in the log2 domain, l)
   int H, KV, S_cap, splits, chunk;
   float scale_log2;
+  int Tq;           // queries per batch row (MULTI only)
 };
 
+// MULTI = false: one query per batch row, tile row g = query head g of this kv head.  MULTI = true: Tq queries per batch
+// row (query j at cache position kv_end - Tq + j), tile row j*G + g; every tile row has its own key limit, so a row sees
+// exactly the keys it would see alone.  Sub-blocks or whole splits past a row's limit are exact no-ops for that row (its
+// scores are -inf: m unchanged, alpha = exp2(0) = 1, p = 0; an untouched split leaves l = 0, which the merge skips).
+template <bool MULTI>
 __global__ void __launch_bounds__(DEC_THREADS, 2) attn_decode_kernel(const DecodeParams p) {
   extern __shared__ __align__(128) uint8_t smem[];
   const uint32_t sb = smem_u32(smem);
@@ -61,10 +72,19 @@ __global__ void __launch_bounds__(DEC_THREADS, 2) attn_decode_kernel(const Decod
   const int hi = min(min(p.kv_end[b], p.S_cap), (split + 1) * p.chunk);
   float* pml = p.part_ml + ((int64_t(b) * p.H + kvh * G) * p.splits + split) * 2;
   float* po = p.part_o + ((int64_t(b) * p.H + kvh * G) * p.splits + split) * ATT_HD;
+  // MULTI: tile row r = j*G + g is partial row [b*Tq + j, kvh*G + g] (element offset of its (m, l) pair / 2)
+  const auto part = [&](int r) { return ((int64_t(b) * p.Tq + r / G) * p.H + kvh * G + r % G) * p.splits + split; };
   if (hi <= lo) {   // nothing of this row's range in this chunk: an empty partial
-    for (int g = tid; g < G; g += DEC_THREADS) {
-      pml[int64_t(g) * p.splits * 2] = -INFINITY;
-      pml[int64_t(g) * p.splits * 2 + 1] = 0.f;
+    if constexpr (MULTI) {
+      for (int r = tid; r < p.Tq * G; r += DEC_THREADS) {
+        p.part_ml[part(r) * 2] = -INFINITY;
+        p.part_ml[part(r) * 2 + 1] = 0.f;
+      }
+    } else {
+      for (int g = tid; g < G; g += DEC_THREADS) {
+        pml[int64_t(g) * p.splits * 2] = -INFINITY;
+        pml[int64_t(g) * p.splits * 2 + 1] = 0.f;
+      }
     }
     return;
   }
@@ -74,8 +94,17 @@ __global__ void __launch_bounds__(DEC_THREADS, 2) attn_decode_kernel(const Decod
   const int nsub = (hi - kbase + ATT_SUB - 1) / ATT_SUB;
   const uint32_t sQ = sb, sK0 = sb + DEC_Q_TILE, sV0 = sK0 + DEC_STAGES * DEC_SUB_TILE;
 
-  // the G query heads of this kv head are rows 0..G-1 of a 16-row tile (rows >= G zero)
-  load_tile_async<16, DEC_THREADS>(sQ, p.Q + int64_t(b) * p.ldq + int64_t(kvh) * G * ATT_HD, ATT_HD, 0, 0, G, tid);
+  if constexpr (MULTI) {   // tile row j*G + g <- head kvh*G + g of query row b*Tq + j (rows >= Tq*G zero)
+    for (int i = tid; i < 16 * 16; i += DEC_THREADS) {
+      const int r = i >> 4, ch = i & 15;
+      const bool ok = r < p.Tq * G;
+      const bf16* src =
+          p.Q + (ok ? (int64_t(b) * p.Tq + r / G) * p.ldq + int64_t(kvh * G + r % G) * ATT_HD : 0) + ch * 8;
+      cp_async16(sQ + tile_off(r, ch), src, ok ? 16u : 0u);
+    }
+  } else {                 // the G query heads of this kv head are rows 0..G-1 of a 16-row tile (rows >= G zero)
+    load_tile_async<16, DEC_THREADS>(sQ, p.Q + int64_t(b) * p.ldq + int64_t(kvh) * G * ATT_HD, ATT_HD, 0, 0, G, tid);
+  }
   auto load_stage = [&](int i) {
     if (i < nsub) {
       const int st = i % DEC_STAGES, k0 = kbase + i * ATT_SUB;
@@ -108,11 +137,21 @@ __global__ void __launch_bounds__(DEC_THREADS, 2) attn_decode_kernel(const Decod
 
     float s[2][4];
     mma_scores_nk<1>(s, qf, sK, warp * 16);
-    const auto mask = [&](float x, int j, int e) {
-      const int key = k0 + 8 * j + cq + (e & 1);
-      return (key >= lo && key < hi) ? x * p.scale_log2 : -INFINITY;
-    };
-    softmax_step(s, mask, o, m_a, m_b, l_a, l_b);
+    if constexpr (MULTI) {   // per-row key limits: query j sees cache rows < kv_end - Tq + j + 1
+      const int hi_a = min(hi, p.kv_end[b] - p.Tq + (lane >> 2) / G + 1);
+      const int hi_b = min(hi, p.kv_end[b] - p.Tq + ((lane >> 2) + 8) / G + 1);
+      const auto mask = [&](float x, int j, int e) {
+        const int key = k0 + 8 * j + cq + (e & 1);
+        return (key >= lo && key < (e < 2 ? hi_a : hi_b)) ? x * p.scale_log2 : -INFINITY;
+      };
+      softmax_step(s, mask, o, m_a, m_b, l_a, l_b);
+    } else {
+      const auto mask = [&](float x, int j, int e) {
+        const int key = k0 + 8 * j + cq + (e & 1);
+        return (key >= lo && key < hi) ? x * p.scale_log2 : -INFINITY;
+      };
+      softmax_step(s, mask, o, m_a, m_b, l_a, l_b);
+    }
     mma_acc_kn(o, s, sV, warp * 16);
   }
   cp_async_wait<0>();
@@ -136,7 +175,7 @@ __global__ void __launch_bounds__(DEC_THREADS, 2) attn_decode_kernel(const Decod
     sL[warp * 16 + ra] = l_a; sL[warp * 16 + ra + 8] = l_b;
   }
   __syncthreads();
-  for (int i = tid; i < G * ATT_HD; i += DEC_THREADS) {
+  for (int i = tid; i < (MULTI ? p.Tq * G : G) * ATT_HD; i += DEC_THREADS) {   // tile rows in use
     const int g = i / ATT_HD, c = i % ATT_HD;
     float M = -INFINITY;
 #pragma unroll
@@ -149,10 +188,18 @@ __global__ void __launch_bounds__(DEC_THREADS, 2) attn_decode_kernel(const Decod
       acc += f * sO[(w * 16 + g) * ATT_HD + c];
       L += f * sL[w * 16 + g];
     }
-    po[int64_t(g) * p.splits * ATT_HD + c] = acc;
-    if (c == 0) {
-      pml[int64_t(g) * p.splits * 2] = M;
-      pml[int64_t(g) * p.splits * 2 + 1] = L;
+    if constexpr (MULTI) {
+      p.part_o[part(g) * ATT_HD + c] = acc;
+      if (c == 0) {
+        p.part_ml[part(g) * 2] = M;
+        p.part_ml[part(g) * 2 + 1] = L;
+      }
+    } else {
+      po[int64_t(g) * p.splits * ATT_HD + c] = acc;
+      if (c == 0) {
+        pml[int64_t(g) * p.splits * 2] = M;
+        pml[int64_t(g) * p.splits * 2 + 1] = L;
+      }
     }
   }
 }
@@ -220,22 +267,28 @@ __device__ __forceinline__ bool argmax_better(float x, int i, float best, int bi
   return i < bi;
 }
 
-// The body of both selection kernels.  Logits row r selects for slot b (r == b without a slot map).  SLOTS = false is
-// tn_greedy_select_bf16: every row advances, finished rows take pad.  SLOTS = true is tn_greedy_select_slots_bf16: a
+enum SelectMode { SEL_PLAIN, SEL_SLOTS, SEL_VERIFY };
+
+// The body of the three selection kernels.  Logits row r selects for slot b (r == b without a slot map).  SEL_PLAIN is
+// tn_greedy_select_bf16: every row advances, finished rows take pad.  SEL_SLOTS is tn_greedy_select_slots_bf16: a
 // finished (or idle) slot does not advance at all (pad in next_ids, nothing else written), and a slot also finishes
-// when its length reaches limit[b].
-template <bool SLOTS>
+// when its length reaches limit[b].  SEL_VERIFY is position `extra` of a speculative block (tn_verify_select_bf16): the
+// history is row b followed by the draft tokens draft[0 .. extra), a finished row picks nothing, and the pick goes to
+// *pick instead of the decoding state.
+template <int MODE>
 __device__ __forceinline__ void greedy_select_row(
     const bf16* __restrict__ logits, int64_t ld, int V, int64_t* __restrict__ history, int64_t ld_hist,
     int32_t* __restrict__ length, int64_t* __restrict__ positions, int64_t* __restrict__ next_ids,
     int32_t* __restrict__ finished, const int32_t* __restrict__ limit, float penalty, int ngram, int64_t eos,
-    int64_t pad, const int r, const int b) {
+    int64_t pad, const int r, const int b, const int64_t* __restrict__ draft = nullptr, int extra = 0,
+    int64_t* __restrict__ pick = nullptr) {
+  constexpr bool SLOTS = MODE == SEL_SLOTS, VERIFY = MODE == SEL_VERIFY;
   extern __shared__ uint32_t bits[];   // [2][words]: repetition set, banned set
   __shared__ float s_val[SEL_THREADS / 32];
   __shared__ int s_idx[SEL_THREADS / 32];
   const int tid = threadIdx.x;
-  if (SLOTS && finished[b]) {          // uniform over the CTA: no barrier has been reached yet
-    if (tid == 0) next_ids[b] = pad;
+  if ((SLOTS || VERIFY) && finished[b]) {   // uniform over the CTA: no barrier has been reached yet
+    if (tid == 0 && SLOTS) next_ids[b] = pad;
     return;
   }
   const int words = (V + 31) / 32;
@@ -243,12 +296,14 @@ __device__ __forceinline__ void greedy_select_row(
   uint32_t* ban = bits + words;
   for (int i = tid; i < 2 * words; i += SEL_THREADS) bits[i] = 0u;
   __syncthreads();
-  const int len = length[b];
-  const int64_t* h = history + int64_t(b) * ld_hist;
+  const int n0 = length[b];
+  const int len = n0 + extra;
+  const int64_t* h0 = history + int64_t(b) * ld_hist;
+  const auto h = [&](int i) { return VERIFY && i >= n0 ? draft[i - n0] : h0[i]; };
   const bool use_pen = penalty != 1.0f;
   if (use_pen) {
     for (int i = tid; i < len; i += SEL_THREADS) {
-      const int64_t id = h[i];
+      const int64_t id = h(i);
       if (id >= 0 && id < V) atomicOr(&rep[id >> 5], 1u << (id & 31));
     }
   }
@@ -256,8 +311,8 @@ __device__ __forceinline__ void greedy_select_row(
     // ngram i = h[i .. i+n-1]; its last id is banned when its first n-1 ids equal the last n-1 ids of the sequence
     for (int i = tid; i + ngram <= len; i += SEL_THREADS) {
       bool match = true;
-      for (int j = 0; j < ngram - 1 && match; ++j) match = h[i + j] == h[len - ngram + 1 + j];
-      const int64_t id = h[i + ngram - 1];
+      for (int j = 0; j < ngram - 1 && match; ++j) match = h(i + j) == h(len - ngram + 1 + j);
+      const int64_t id = h(i + ngram - 1);
       if (match && id >= 0 && id < V) atomicOr(&ban[id >> 5], 1u << (id & 31));
     }
   }
@@ -286,13 +341,17 @@ __device__ __forceinline__ void greedy_select_row(
       const int oi = s_idx[w];
       if (argmax_better(ov, oi, best, bi)) { best = ov; bi = oi; }
     }
-    const int fin = SLOTS ? 0 : finished[b];
-    const int64_t tok = fin ? pad : int64_t(bi);
-    if (len < ld_hist) history[int64_t(b) * ld_hist + len] = tok;
-    next_ids[b] = tok;
-    length[b] = len + 1;
-    positions[b] += 1;
-    if (tok == eos || (SLOTS && len + 1 == limit[b])) finished[b] = 1;
+    if constexpr (VERIFY) {
+      *pick = bi;
+    } else {
+      const int fin = SLOTS ? 0 : finished[b];
+      const int64_t tok = fin ? pad : int64_t(bi);
+      if (len < ld_hist) history[int64_t(b) * ld_hist + len] = tok;
+      next_ids[b] = tok;
+      length[b] = len + 1;
+      positions[b] += 1;
+      if (tok == eos || (SLOTS && len + 1 == limit[b])) finished[b] = 1;
+    }
   }
 }
 
@@ -300,8 +359,52 @@ __global__ void __launch_bounds__(SEL_THREADS) greedy_select_kernel(
     const bf16* __restrict__ logits, int64_t ld, int V, int64_t* __restrict__ history, int64_t ld_hist,
     int32_t* __restrict__ length, int64_t* __restrict__ positions, int64_t* __restrict__ next_ids,
     int32_t* __restrict__ finished, float penalty, int ngram, int64_t eos, int64_t pad) {
-  greedy_select_row<false>(logits, ld, V, history, ld_hist, length, positions, next_ids, finished, nullptr, penalty,
+  greedy_select_row<SEL_PLAIN>(logits, ld, V, history, ld_hist, length, positions, next_ids, finished, nullptr, penalty,
                            ngram, eos, pad, blockIdx.x, blockIdx.x);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// speculative verification: the picks of k + 1 positions (grid (k + 1, B)), then per row the accepted prefix
+// ---------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(SEL_THREADS) verify_pick_kernel(
+    const bf16* __restrict__ logits, int64_t ld, int V, int64_t* __restrict__ history, int64_t ld_hist,
+    int32_t* __restrict__ length, int32_t* __restrict__ finished, const int64_t* __restrict__ draft, int k,
+    int64_t* __restrict__ picks, float penalty, int ngram) {
+  const int j = blockIdx.x, b = blockIdx.y;
+  const int r = b * (k + 1) + j;
+  greedy_select_row<SEL_VERIFY>(logits, ld, V, history, ld_hist, length, nullptr, nullptr, finished, nullptr, penalty,
+                                ngram, 0, 0, r, b, draft + int64_t(b) * k, j, picks + r);
+}
+
+// one thread per row: emit picks 0..n (n = the leading draft tokens equal to their pick), stopping after an eos and at
+// the row's limit, then advance the row's state as the slot selection does for one token
+__global__ void verify_commit_kernel(const int64_t* __restrict__ picks, const int64_t* __restrict__ draft, int k, int B,
+                                     int64_t* __restrict__ history, int64_t ld_hist, int32_t* __restrict__ length,
+                                     int64_t* __restrict__ positions, int64_t* __restrict__ next_ids,
+                                     int32_t* __restrict__ finished, const int32_t* __restrict__ limit, int64_t eos,
+                                     int64_t pad) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  if (finished[b]) {   // a finished row does not advance
+    next_ids[b] = pad;
+    return;
+  }
+  const int len = length[b], lim = limit[b];
+  const int64_t* pk = picks + int64_t(b) * (k + 1);
+  const int64_t* d = draft + int64_t(b) * k;
+  int c = 0;
+  int64_t tok;
+  bool stop;
+  do {
+    tok = pk[c];
+    if (len + c < ld_hist) history[int64_t(b) * ld_hist + len + c] = tok;
+    ++c;
+    stop = tok == eos || len + c >= lim || c == k + 1 || d[c - 1] != tok;
+  } while (!stop);
+  length[b] = len + c;
+  positions[b] += c;
+  next_ids[b] = tok;
+  if (tok == eos || len + c >= lim) finished[b] = 1;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -328,7 +431,7 @@ __global__ void __launch_bounds__(SEL_THREADS, 1) greedy_select_slots_kernel(
     int32_t* __restrict__ finished, const int32_t* __restrict__ limit, float penalty, int ngram, int64_t eos,
     int64_t pad, const SlotMap map) {
   const int r = blockIdx.x;
-  greedy_select_row<true>(logits, ld, V, history, ld_hist, length, positions, next_ids, finished, limit, penalty, ngram,
+  greedy_select_row<SEL_SLOTS>(logits, ld, V, history, ld_hist, length, positions, next_ids, finished, limit, penalty, ngram,
                           eos, pad, r, map.use_map ? map.slot[r] : r);
 }
 
@@ -382,36 +485,63 @@ extern "C" int64_t tn_attn_decode_ws_floats(int B, int H, int KV, int S_cap) {
   return int64_t(B) * H * decode_splits(B, KV, S_cap) * (ATT_HD + 2);
 }
 
-extern "C" int tn_attn_decode_bf16(const void* Q, int64_t ldq, const void* K, const void* V, int64_t ld_tok,
-                                   int64_t ld_batch, const int32_t* kv_start, const int32_t* kv_end, int B, int H, int KV,
-                                   int S_cap, float scale, float* workspace, void* O, int64_t ldo, float* lse,
-                                   tn_stream_t stream_) {
-  clear_error();
+extern "C" int64_t tn_attn_decode_multi_ws_floats(int B, int Tq, int H, int KV, int S_cap) {
+  if (Tq <= 0) return 0;
+  return tn_attn_decode_ws_floats(B, H, KV, S_cap) * Tq;   // the splits of the single-query launch, per query
+}
+
+// both decode attention launches: Tq query rows per batch row (MULTI), the split count and chunking of (B, KV, S_cap)
+template <bool MULTI>
+static int decode_launch(const char* fn, const void* Q, int64_t ldq, const void* K, const void* V, int64_t ld_tok,
+                         int64_t ld_batch, const int32_t* kv_start, const int32_t* kv_end, int B, int Tq, int H, int KV,
+                         int S_cap, float scale, float* workspace, void* O, int64_t ldo, float* lse, tn_stream_t stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  TN_REQUIRE(Q && K && V && kv_start && kv_end && workspace && O, "tn_attn_decode_bf16: null pointer");
+  TN_REQUIRE(Q && K && V && kv_start && kv_end && workspace && O, "%s: null pointer", fn);
   TN_REQUIRE(B > 0 && H > 0 && KV > 0 && S_cap > 0 && H % KV == 0 && H / KV <= 16,
-             "tn_attn_decode_bf16: bad dims B=%d H=%d KV=%d S_cap=%d (H/KV must be 1..16)", B, H, KV, S_cap);
+             "%s: bad dims B=%d H=%d KV=%d S_cap=%d (H/KV must be 1..16)", fn, B, H, KV, S_cap);
   TN_REQUIRE(ldq % 8 == 0 && ld_tok % 8 == 0 && ld_batch % 8 == 0 && ldo % 8 == 0,
-             "tn_attn_decode_bf16: strides must be multiples of 8");
+             "%s: strides must be multiples of 8", fn);
   TN_REQUIRE(ldq >= int64_t(H) * ATT_HD && ldo >= int64_t(H) * ATT_HD && ld_tok >= int64_t(KV) * ATT_HD &&
-                 ld_batch >= ld_tok * S_cap, "tn_attn_decode_bf16: stride smaller than the rows it must hold");
+                 ld_batch >= ld_tok * S_cap, "%s: stride smaller than the rows it must hold", fn);
+  TN_REQUIRE(int64_t(B) * Tq <= 65535, "%s: grid too large (B*Tq = %lld)", fn, (long long)B * Tq);
   const int splits = decode_splits(B, KV, S_cap);
   DecodeParams p{};
   p.Q = static_cast<const bf16*>(Q); p.K = static_cast<const bf16*>(K); p.V = static_cast<const bf16*>(V);
   p.ldq = ldq; p.ld_tok = ld_tok; p.ld_batch = ld_batch;
   p.kv_start = kv_start; p.kv_end = kv_end;
   p.part_o = workspace;
-  p.part_ml = workspace + int64_t(B) * H * splits * ATT_HD;
+  p.part_ml = workspace + int64_t(B) * Tq * H * splits * ATT_HD;
   p.H = H; p.KV = KV; p.S_cap = S_cap; p.splits = splits;
   p.chunk = ((S_cap + splits - 1) / splits + ATT_SUB - 1) / ATT_SUB * ATT_SUB;
   p.scale_log2 = scale * LOG2E;
-  TN_CHECK_CUDA(attn_smem_optin<attn_decode_kernel>(DEC_SMEM));
-  attn_decode_kernel<<<dim3(splits, KV, B), DEC_THREADS, DEC_SMEM, stream>>>(p);
+  p.Tq = Tq;
+  TN_CHECK_CUDA(attn_smem_optin<attn_decode_kernel<MULTI>>(DEC_SMEM));
+  attn_decode_kernel<MULTI><<<dim3(splits, KV, B), DEC_THREADS, DEC_SMEM, stream>>>(p);
   TN_CHECK_CUDA(cudaGetLastError());
-  attn_decode_merge_kernel<<<dim3(H, B), ATT_HD, 0, stream>>>(p.part_o, p.part_ml, static_cast<bf16*>(O), ldo, lse, H,
-                                                              splits);
+  attn_decode_merge_kernel<<<dim3(H, B * Tq), ATT_HD, 0, stream>>>(p.part_o, p.part_ml, static_cast<bf16*>(O), ldo, lse,
+                                                                   H, splits);
   TN_CHECK_CUDA(cudaGetLastError());
   return TN_OK;
+}
+
+extern "C" int tn_attn_decode_bf16(const void* Q, int64_t ldq, const void* K, const void* V, int64_t ld_tok,
+                                   int64_t ld_batch, const int32_t* kv_start, const int32_t* kv_end, int B, int H, int KV,
+                                   int S_cap, float scale, float* workspace, void* O, int64_t ldo, float* lse,
+                                   tn_stream_t stream_) {
+  clear_error();
+  return decode_launch<false>("tn_attn_decode_bf16", Q, ldq, K, V, ld_tok, ld_batch, kv_start, kv_end, B, 1, H, KV,
+                              S_cap, scale, workspace, O, ldo, lse, stream_);
+}
+
+extern "C" int tn_attn_decode_multi_bf16(const void* Q, int64_t ldq, const void* K, const void* V, int64_t ld_tok,
+                                         int64_t ld_batch, const int32_t* kv_start, const int32_t* kv_end, int B, int Tq,
+                                         int H, int KV, int S_cap, float scale, float* workspace, void* O, int64_t ldo,
+                                         float* lse, tn_stream_t stream_) {
+  clear_error();
+  TN_REQUIRE(Tq > 0 && KV > 0 && H % KV == 0 && int64_t(Tq) * (H / KV) <= 16 && Tq <= S_cap,
+             "tn_attn_decode_multi_bf16: bad dims Tq=%d H=%d KV=%d S_cap=%d (Tq*H/KV must be 1..16)", Tq, H, KV, S_cap);
+  return decode_launch<true>("tn_attn_decode_multi_bf16", Q, ldq, K, V, ld_tok, ld_batch, kv_start, kv_end, B, Tq, H, KV,
+                             S_cap, scale, workspace, O, ldo, lse, stream_);
 }
 
 // the checks of both K/V copies (`map`: row_end or the admission table): pointers, dims, strides, 16-byte alignment
@@ -446,7 +576,7 @@ extern "C" int tn_kv_append_bf16(const void* K, int64_t ldk, const void* V, int6
 
 // both selection launches, one CTA per logits row: processor arguments, bitmap bytes, one-time shared-memory opt-in
 template <auto kernel, typename... Args>
-static int select_launch(const char* fn, int rows, int V, float penalty, int ngram, tn_stream_t stream, Args... args) {
+static int select_launch(const char* fn, dim3 rows, int V, float penalty, int ngram, tn_stream_t stream, Args... args) {
   TN_REQUIRE(penalty > 0.f, "%s: repetition_penalty must be > 0", fn);
   TN_REQUIRE(ngram >= 0, "%s: no_repeat_ngram_size must be >= 0", fn);
   const size_t smem = size_t(2) * ((V + 31) / 32) * sizeof(uint32_t);
@@ -500,6 +630,28 @@ extern "C" int tn_greedy_select_slots_bf16(const void* logits, int64_t ld, int n
       "tn_greedy_select_slots_bf16", n_rows, V, repetition_penalty, no_repeat_ngram_size, stream_,
       static_cast<const bf16*>(logits), ld, V, history, ld_hist, length, positions, next_ids, finished, limit,
       repetition_penalty, no_repeat_ngram_size, eos, pad, map);
+}
+
+extern "C" int tn_verify_select_bf16(const void* logits, int64_t ld, int B, int k, int V, const int64_t* draft,
+                                     int64_t* history, int64_t ld_hist, int32_t* length, int64_t* positions,
+                                     int64_t* next_ids, int32_t* finished, const int32_t* limit, int64_t* picks,
+                                     float repetition_penalty, int no_repeat_ngram_size, int64_t eos, int64_t pad,
+                                     tn_stream_t stream_) {
+  clear_error();
+  TN_REQUIRE(logits && draft && history && length && positions && next_ids && finished && limit && picks,
+             "tn_verify_select_bf16: null pointer");
+  TN_REQUIRE(B > 0 && k > 0 && V > 0 && ld >= V && ld_hist > 0, "tn_verify_select_bf16: bad dims B=%d k=%d V=%d", B, k,
+             V);
+  TN_REQUIRE(B <= 65535 && k < 65535, "tn_verify_select_bf16: grid too large (B=%d, k=%d)", B, k);
+  const int rc = select_launch<verify_pick_kernel>(
+      "tn_verify_select_bf16", dim3(k + 1, B), V, repetition_penalty, no_repeat_ngram_size, stream_,
+      static_cast<const bf16*>(logits), ld, V, history, ld_hist, length, finished, draft, k, picks, repetition_penalty,
+      no_repeat_ngram_size);
+  if (rc != TN_OK) return rc;
+  verify_commit_kernel<<<(B + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream_)>>>(
+      picks, draft, k, B, history, ld_hist, length, positions, next_ids, finished, limit, eos, pad);
+  TN_CHECK_CUDA(cudaGetLastError());
+  return TN_OK;
 }
 
 // docs: host [n_docs][4] int32 = (src_row, slot, len, limit); checked against the cache shape, returned by value

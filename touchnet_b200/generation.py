@@ -16,6 +16,10 @@ repetition_penalty, no_repeat_ngram_size, max_new_tokens, ...)` on left-padded p
            continuous batching over many prompts: a cache of B slots, finished rows refilled with the next prompts
            (packed prefill into chosen slots: tn_kv_scatter_bf16, tn_slot_admit) while the captured decode step keeps
            replaying (tn_greedy_select_slots_bf16 holds finished and idle slots still).
+  speculative
+           generate(assistant_model=draft): per round the draft proposes k tokens, the model scores them in one step of
+           B*(k+1) rows (tn_attn_decode_multi_bf16) and keeps the longest prefix equal to its own picks plus its next
+           pick (tn_verify_select_bf16); the output is bit-identical to generate without the draft.
 
 The new tokens belong to the last document of each row: the decode query of row b attends to cache rows
 [kv_start[b], kv_end[b]) with kv_start[b] the first position of the row's last document in the prompt's attention_mask
@@ -179,13 +183,14 @@ def _prompt_front(model, w: _Weights, input_ids, input_features, doc, pos):
     return (x, ops.AttnPlan(doc), *ops.rope_table(pos, w.inv_freq, w.rope_scaling))
 
 
-def _layers(cache: B200KVCache, w: _Weights, x, cos, sin, attend):
+def _layers(cache: B200KVCache, w: _Weights, x, cos, sin, attend, qkv_rows=None):
     """Every block over the rows x; `attend(q, k, v, k_cache, v_cache) -> (o, lse)` stores the layer's K/V into its
-    cache and runs the attention."""
+    cache and runs the attention.  `qkv_rows`: see ops.block_forward."""
     for i, lw in enumerate(w.layers):
         kc, vc = cache.layer(i)
         x, _ = ops.block_forward(x, *lw, cos, sin, cache.H, cache.KV, w.eps, cache.hd,
-                                 lambda q, k, v, kc=kc, vc=vc: (*attend(q, k, v, kc, vc), k, v), need_gu=False)
+                                 lambda q, k, v, kc=kc, vc=vc: (*attend(q, k, v, kc, vc), k, v), need_gu=False,
+                                 qkv_rows=qkv_rows)
     return x
 
 
@@ -303,14 +308,19 @@ def _captured(step, capture: bool):
     return run
 
 
-def _host_sync(flags, nan_flag) -> list:
-    """The one host sync per decode step: the int32 tensors `flags` and the NaN flag read in one `.tolist()`.  A set NaN
-    flag is zeroed and raises ValueError; otherwise returns the values of `flags`, flattened."""
-    flags = [f.reshape(-1) for f in flags] + ([] if nan_flag is None else [nan_flag])
+def _host_sync(flags, *nan_flags) -> list:
+    """The one host sync per decode step: the int32 tensors `flags` and the NaN flags (None: no flag) read in one
+    `.tolist()`.  A set NaN flag is zeroed and raises ValueError; otherwise returns the values of `flags`, flattened."""
+    nan_flags = [f for f in nan_flags if f is not None]
+    flags = [f.reshape(-1) for f in flags] + nan_flags
     vals = (flags[0] if len(flags) == 1 else torch.cat(flags)).tolist()
-    if nan_flag is not None and vals.pop() != 0:
-        nan_flag.zero_()
-        raise ValueError("NaN in data.")
+    if nan_flags:
+        bad = vals[len(vals) - len(nan_flags):]
+        del vals[len(vals) - len(nan_flags):]
+        if any(bad):
+            for f in nan_flags:
+                f.zero_()
+            raise ValueError("NaN in data.")
     return vals
 
 
@@ -318,7 +328,16 @@ def generate(model, input_ids, input_features=None, attention_mask=None, positio
              eos_token_id, pad_token_id, repetition_penalty=1.0, no_repeat_ngram_size=0, do_sample=False, num_beams=1,
              use_cache=True, bos_token_id=None, top_k=None, top_p=None, temperature=None, early_stopping=None, **kwargs):
     """Greedy decoding with HF `generate` semantics: returns [B, T + n] ids (the prompt, then n <= max_new_tokens
-    generated ids; rows that emitted eos continue with pad), stopping when every row has emitted eos."""
+    generated ids; rows that emitted eos continue with pad), stopping when every row has emitted eos.
+    With `assistant_model` (HF's assisted generation) a draft model proposes `num_assistant_tokens` tokens per round
+    and the model verifies them in one step (see generate_speculative): the result is the same tensor, bit for bit."""
+    if kwargs.get("assistant_model") is not None:
+        return generate_speculative(
+            model, input_ids, input_features, attention_mask, position_ids, max_new_tokens=max_new_tokens,
+            eos_token_id=eos_token_id, pad_token_id=pad_token_id, repetition_penalty=repetition_penalty,
+            no_repeat_ngram_size=no_repeat_ngram_size, do_sample=do_sample, num_beams=num_beams, use_cache=use_cache,
+            bos_token_id=bos_token_id, top_k=top_k, top_p=top_p, temperature=temperature, early_stopping=early_stopping,
+            **kwargs)
     _validate(max_new_tokens, eos_token_id, pad_token_id, repetition_penalty, no_repeat_ngram_size, do_sample, num_beams,
               kwargs)
     _check_scope(model)
@@ -346,6 +365,166 @@ def generate(model, input_ids, input_features=None, attention_mask=None, positio
         if n == max_new and nan_flag is not None:
             _host_sync([], nan_flag)
     return cache.history[:, :T + n].clone()
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# speculative decoding (HF assisted generation): a draft model proposes, the model verifies k + 1 rows in one step
+# ---------------------------------------------------------------------------------------------------------------
+# assisted-generation knobs of HF `generate` that are not implemented (a fixed number of draft tokens per round only)
+_SPEC_UNSUPPORTED = ("assistant_confidence_threshold", "prompt_lookup_num_tokens", "assistant_early_exit",
+                     "assistant_tokenizer")
+
+
+def _gqa(model) -> int:
+    a = _parts(model)[0].model.layers[0].self_attn
+    return a.num_heads // a.num_key_value_heads
+
+
+def _spec_args(model, draft, k, schedule, kwargs) -> int:
+    """Checks of the draft and of the assisted-generation arguments; returns the number of draft tokens per round."""
+    bad = sorted(n for n in _SPEC_UNSUPPORTED if kwargs.pop(n, None) is not None)
+    if bad:
+        raise TouchNetB200Error(f"generate: unsupported assisted-generation arguments {bad} (a fixed number of draft "
+                                "tokens per round only)")
+    if schedule is not None and schedule != "constant":
+        raise TouchNetB200Error(f"generate: num_assistant_tokens_schedule must be 'constant', got {schedule!r}")
+    lm, audio = _parts(model)
+    dlm, daudio = _parts(draft)
+    if not isinstance(dlm, type(lm)) or (audio is None) != (daudio is None):
+        raise TouchNetB200Error("generate: the assistant_model must be a B200 model of the same kind as the model "
+                                "(both Llama, or both TouchAudio)")
+    if audio is not None and daudio.projector.weight.shape[1] != audio.projector.weight.shape[1]:
+        raise TouchNetB200Error("generate: the assistant_model's projector input width differs from the model's")
+    if dlm.config.vocab_size != lm.config.vocab_size:
+        raise TouchNetB200Error(f"generate: the assistant_model's vocab_size {dlm.config.vocab_size} differs from the "
+                                f"model's {lm.config.vocab_size}")
+    if dlm.lm_head.weight.device != lm.lm_head.weight.device:
+        raise TouchNetB200Error("generate: the assistant_model is on another device")
+    _check_scope(draft)
+    G, Gd = _gqa(model), _gqa(draft)
+    if k is None and G > 8:
+        raise TouchNetB200Error(f"generate: the model's H/KV = {G} leaves no room for a draft token: its verify step "
+                                "needs H/KV * (num_assistant_tokens + 1) <= 16")
+    k = min(4, 16 // G - 1) if k is None else k
+    if isinstance(k, bool) or int(k) != k or int(k) < 1:
+        raise TouchNetB200Error(f"generate: num_assistant_tokens must be an int >= 1, got {k}")
+    k = int(k)
+    if G * (k + 1) > 16:
+        raise TouchNetB200Error(f"generate: num_assistant_tokens {k} with H/KV = {G}: the verify step needs "
+                                "H/KV * (num_assistant_tokens + 1) <= 16")
+    if 2 * Gd > 16:
+        raise TouchNetB200Error(f"generate: the assistant_model's H/KV = {Gd}: its two-token step needs 2 * H/KV <= 16")
+    return k
+
+
+def _block_step(model, cache: B200KVCache, w: _Weights, ids, pos, end, workspace, s_attn: int):
+    """Tq = ids.shape[1] new tokens per row: ids / pos [B, Tq] at cache rows [end - Tq, end) (K/V appended there),
+    query j attending to [kv_start, end - Tq + j + 1).  Returns the last hidden state [B*Tq, d].  Every row is computed
+    as decode_step computes its token: the QKV path is chosen for B rows, and the attention runs on cache rows
+    [0, s_attn) only, so that its split count and chunks (functions of the cache length) are those of a decode step
+    on a cache of s_attn rows; a query whose range reaches past s_attn is clipped there."""
+    _, audio = _parts(model)
+    B, Tq = ids.shape
+    x = ops.embed_add(ids.reshape(-1), w.embed, None, B * Tq, w.embed.shape[1], None if audio is None else audio._nan_flag)
+    cos, sin = ops.rope_table(pos, w.inv_freq, w.rope_scaling)
+
+    def attend(q, k, v, kc, vc):
+        ops.kv_append(k, v, kc, vc, end, Tq)
+        return ops.attn_decode_multi(q, kc[:, :s_attn], vc[:, :s_attn], cache.kv_start, end, Tq, cache.H, cache.KV,
+                                     cache.scale, workspace), None
+
+    return _layers(cache, w, x, cos, sin, attend, qkv_rows=B)
+
+
+def _multi_ws(cache: B200KVCache, Tq: int, s_attn: int) -> torch.Tensor:
+    n = _lib.load().tn_attn_decode_multi_ws_floats(cache.B, Tq, cache.H, cache.KV, s_attn)
+    return torch.empty(int(n), dtype=torch.float32, device=cache.data.device)
+
+
+def generate_speculative(model, input_ids, input_features=None, attention_mask=None, position_ids=None, *,
+                         assistant_model, max_new_tokens, eos_token_id, pad_token_id, num_assistant_tokens=None,
+                         num_assistant_tokens_schedule=None, repetition_penalty=1.0, no_repeat_ngram_size=0,
+                         do_sample=False, num_beams=1, use_cache=True, bos_token_id=None, top_k=None, top_p=None,
+                         temperature=None, early_stopping=None, **kwargs):
+    """`generate(..., assistant_model=draft, num_assistant_tokens=k)`: returns exactly what `generate` returns without
+    the draft.  Each round the draft proposes k tokens per row (its own greedy picks with the same processors), the
+    model scores next_ids and the k proposals in ONE step of B*(k+1) rows (multi-query decode attention) and keeps the
+    longest prefix of proposals equal to its own picks plus its next pick (tn_verify_select_bf16).  Since position j of
+    that step computes exactly what decode_step computes for the same prefix, the picks are the greedy picks; the draft
+    changes how many tokens a round yields, never which.
+
+    The draft receives the same prompt (ids, features, mask, positions).  A round is captured once as a CUDA graph:
+    bring the draft's state to the accepted prefix, a two-token draft step (the last two accepted tokens: the draft
+    never fed its last proposal when all were accepted), k - 1 one-token draft steps, the verify step; then one host sync
+    reads the finished flags and both NaN flags."""
+    k = _spec_args(model, assistant_model, num_assistant_tokens, num_assistant_tokens_schedule, kwargs)
+    _validate(max_new_tokens, eos_token_id, pad_token_id, repetition_penalty, no_repeat_ngram_size, do_sample, num_beams,
+              kwargs)
+    _check_scope(model)
+    eos, pad = int(eos_token_id), int(pad_token_id)
+    penalty, ngram = float(repetition_penalty), int(no_repeat_ngram_size)
+    draft = assistant_model
+    lm, audio = _parts(model)
+    dlm, daudio = _parts(draft)
+    B, T = input_ids.shape
+    if attention_mask is not None:
+        _check_mask(attention_mask, B, T)
+    max_new = int(max_new_tokens)
+    dev = input_ids.device
+    with torch.no_grad():
+        w, wd = _Weights(lm), _Weights(dlm)
+        S_cap = T + max_new + k              # the verify step writes up to k rows past the final length
+        # ... but attends as `generate` does on its cache of T + max_new rows: the same decode splits and chunks.
+        # A query row clipped there lies past `limit`, so its pick is never emitted.
+        S_gen = T + max_new
+        tc = B200KVCache(model, B, S_cap, device=dev)
+        dc = B200KVCache(draft, B, S_cap, device=dev)
+        flags = (None if audio is None else audio._nan_flag, None if daudio is None else daudio._nan_flag)
+        limit = torch.full((B,), T + max_new, dtype=torch.int32, device=dev)
+        drafts = torch.zeros((B, k), dtype=torch.int64, device=dev)
+        picks = torch.zeros((B, k + 1), dtype=torch.int64, device=dev)
+        end = torch.zeros(B, dtype=torch.int32, device=dev)
+        ar = torch.arange(k + 1, dtype=torch.int64, device=dev)
+        ws, dws = _multi_ws(tc, k + 1, S_gen), _multi_ws(dc, 2, S_cap)
+
+        ops.greedy_select(prefill(model, tc, input_ids, input_features, attention_mask, position_ids, weights=w),
+                          tc.history, tc.kv_end, tc.positions, tc.next_ids, tc.finished, penalty, ngram, eos, pad)
+        prefill(draft, dc, input_ids, input_features, attention_mask, position_ids, weights=wd)
+
+        def draft_select(logits, j):
+            ops.greedy_select(logits, dc.history, dc.kv_end, dc.positions, dc.next_ids, dc.finished, penalty, ngram,
+                              eos, pad)
+            drafts[:, j].copy_(dc.next_ids)
+
+        def round_():
+            for dst, src in ((dc.history, tc.history), (dc.kv_end, tc.kv_end), (dc.positions, tc.positions),
+                             (dc.finished, tc.finished)):
+                dst.copy_(src)
+            # the last two accepted tokens, at positions - 1 and positions
+            ids2 = dc.history.gather(1, dc.kv_end.to(torch.int64)[:, None] - 2 + ar[None, :2])
+            x = _block_step(draft, dc, wd, ids2, dc.positions[:, None] - 1 + ar[None, :2], dc.kv_end, dws, S_cap)
+            draft_select(_logits_last(wd, x.view(B, 2, -1)[:, 1].contiguous()), 0)
+            for j in range(1, k):
+                draft_select(decode_step(draft, dc, weights=wd), j)
+            # verify: next_ids and the k proposals at positions + 0..k, appended at rows [kv_end - 1, kv_end + k)
+            torch.add(tc.kv_end, k, out=end)
+            x = _block_step(model, tc, w, torch.cat([tc.next_ids[:, None], drafts], 1), tc.positions[:, None] + ar,
+                            end, ws, S_gen)
+            ops.verify_select(_logits_last(w, x), drafts, tc.history, tc.kv_end, tc.positions, tc.next_ids,
+                              tc.finished, limit, penalty, ngram, eos, pad, picks=picks)
+
+        step = _captured(round_, input_ids.is_cuda)
+        if max_new == 1:
+            _host_sync([tc.finished.min()], *flags)
+        else:
+            while not _host_sync([tc.finished.min()], *flags)[0]:
+                step()
+        count = (tc.kv_end - T).tolist()
+        n = min(max_new, max(count))
+        out = tc.history[:, :T + n].clone()
+        beyond = torch.arange(n, device=dev)[None, :] >= torch.tensor(count, device=dev)[:, None]
+        out[:, T:].masked_fill_(beyond, pad)
+    return out
 
 
 # ---------------------------------------------------------------------------------------------------------------

@@ -397,6 +397,26 @@ def attn_decode(q, k_cache, v_cache, kv_start, kv_end, H: int, KV: int, scale: f
     return (o, lse_t) if lse else o
 
 
+def attn_decode_multi(q, k_cache, v_cache, kv_start, kv_end, Tq: int, H: int, KV: int, scale: float, workspace=None,
+                      lse: bool = False):
+    """attn_decode for Tq new rows per batch row: q [B*Tq, H*128], row b*Tq + j at cache position kv_end[b] - Tq + j,
+    attends to cache rows [kv_start[b], kv_end[b] - Tq + j + 1) -> o [B*Tq, H*128] (and lse [B*Tq, H]); each row is
+    bit-identical to attn_decode at its own length."""
+    _chk(q, "q", BF16); _chk(k_cache, "k_cache", BF16); _chk(v_cache, "v_cache", BF16)
+    B, S_cap = k_cache.shape[0], k_cache.shape[1]
+    assert k_cache.stride() == v_cache.stride() and k_cache.stride(2) == 1 and q.stride(1) == 1
+    if workspace is None:
+        workspace = torch.empty(int(_lib.load().tn_attn_decode_multi_ws_floats(B, Tq, H, KV, S_cap)),
+                                dtype=torch.float32, device=q.device)
+    o = torch.empty((B * Tq, H * 128), dtype=BF16, device=q.device)
+    lse_t = torch.empty((B * Tq, H), dtype=torch.float32, device=q.device) if lse else None
+    _lib.call("tn_attn_decode_multi_bf16", q.data_ptr(), q.stride(0), k_cache.data_ptr(), v_cache.data_ptr(),
+              k_cache.stride(1), k_cache.stride(0), kv_start.data_ptr(), kv_end.data_ptr(), B, int(Tq), H, KV, S_cap,
+              float(scale), workspace.data_ptr(), o.data_ptr(), o.stride(0), None if lse_t is None else lse_t.data_ptr(),
+              _st())
+    return (o, lse_t) if lse else o
+
+
 def _kv_copy_dims(k, v, k_cache, v_cache):
     """The checks both K/V copies make; returns the cache's (B, S_cap, width)."""
     _chk(k, "k", BF16); _chk(v, "v", BF16); _chk(k_cache, "k_cache", BF16)
@@ -432,6 +452,24 @@ def greedy_select(logits, history, length, positions, next_ids, finished, repeti
     _lib.call("tn_greedy_select_bf16", logits.data_ptr(), logits.stride(0), B, V, history.data_ptr(), history.stride(0),
               length.data_ptr(), positions.data_ptr(), next_ids.data_ptr(), finished.data_ptr(),
               float(repetition_penalty), int(no_repeat_ngram_size), int(eos), int(pad), _st())
+
+
+def verify_select(logits, draft, history, length, positions, next_ids, finished, limit, repetition_penalty: float,
+                  no_repeat_ngram_size: int, eos: int, pad: int, picks=None):
+    """Speculative verification over logits [B*(k+1), V] and the draft tokens draft [B, k]: position j's greedy pick
+    over the history extended by draft[:, :j], then per row the accepted prefix plus one token (cut after eos and at
+    limit) written into the decoding state.  Returns picks [B, k+1] (rows not finished)."""
+    n, V = _select_dims(logits, history, length, positions, next_ids, finished)
+    _chk(draft, "draft", torch.int64); _chk(limit, "limit", torch.int32)
+    B, k = draft.shape
+    assert n == B * (k + 1) and history.shape[0] == B and draft.is_contiguous()
+    if picks is None:
+        picks = torch.empty((B, k + 1), dtype=torch.int64, device=logits.device)
+    _lib.call("tn_verify_select_bf16", logits.data_ptr(), logits.stride(0), B, k, V, draft.data_ptr(),
+              history.data_ptr(), history.stride(0), length.data_ptr(), positions.data_ptr(), next_ids.data_ptr(),
+              finished.data_ptr(), limit.data_ptr(), picks.data_ptr(), float(repetition_penalty),
+              int(no_repeat_ngram_size), int(eos), int(pad), _st())
+    return picks
 
 
 def _host_i32(rows) -> torch.Tensor:
@@ -636,17 +674,20 @@ def _unpad_heads(x: torch.Tensor, heads: int, hd: int) -> torch.Tensor:
 
 
 def block_forward(x2, ln1, wqb, wkb, wvb, bq, bk, bv, wob, ln2, wgb, wub, wdb, cos, sin, H, KV, eps, hd, attend, tp=None,
-                  need_gu=True):
+                  need_gu=True, qkv_rows=None):
     """Forward of one pre-norm decoder block on rows x2 [M, d] with bf16 working weights - the body shared by training
     (DecoderLayerFn), prompt prefill and cached decoding (generation.py), which differ only in `attend(q, k, v) ->
     (o, lse, k, v)`: q/k/v arrive projected, rotated and (head_dim < 128) zero-padded to 128-wide heads.
+    `qkv_rows` (default M) is the row count the QKV path (fused with the RoPE epilogue, or not) is chosen for: a
+    speculative verify step passes the decode step's B so that every row is computed as the decode step computes it.
     Returns (out, saved) with saved = (rstd1, h1, q, k, v, o, lse, x1, rstd2, h2, g, u, hm) for the backward."""
     h1, _, rstd1 = rmsnorm_fwd(x2, ln1, eps)
     if tp is not None:
         h1 = tp.gather_rows(h1, keep=True)                               # [B*T, d]: every row, for the local heads
     nq, nkv = wqb.shape[0], wkb.shape[0]
-    rope_in_gemm = qkv_fusable(h1.shape[0], nq, nkv) and bq is None and hd == 128   # RoPE in the QKV GEMM epilogue
-    if qkv_fusable(h1.shape[0], nq, nkv):
+    rows = h1.shape[0] if qkv_rows is None else qkv_rows
+    rope_in_gemm = qkv_fusable(rows, nq, nkv) and bq is None and hd == 128   # RoPE in the QKV GEMM epilogue
+    if qkv_fusable(rows, nq, nkv):
         qkv = gemm_qkv_fwd(h1, wqb, wkb, wvb, rope=(cos, sin) if rope_in_gemm else None)
         q, k, v = qkv[:, :nq], qkv[:, nq:nq + nkv], qkv[:, nq + nkv:]
     else:
