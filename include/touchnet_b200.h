@@ -76,6 +76,41 @@ int tn_gemm_qkv_bf16(int mode, const void* A, int64_t lda, const void* B0, const
                      void* D0, void* D1, void* D2, int64_t ldd, int d_f32, int s0, int s1, int s2, int M, int N, int K,
                      const void* rope_cos, const void* rope_sin, tn_stream_t stream);
 
+/* FP8 twins of the four GEMM entry points above (torchao's tensorwise recipe, opt-in through the model config key
+ * `float8_training`).  Same arguments without the *_mn flags: every operand is K-major 8-bit (A e4m3, or e5m2 when
+ * a_e5m2 / x_e5m2 / dy_e5m2 is set; B always e4m3), and two device floats 1/s_a, 1/s_b (tn_fp8_cast_bf16) multiply the
+ * fp32 accumulator ahead of the epilogue.  An e4m3 A (forward) accumulates in the tensor-core accumulator alone; an e5m2
+ * A (dgrad, wgrad) adds each 128-k partial sum into a separate fp32 accumulator.  All dimensions and leading dimensions
+ * are multiples of 16.
+ *   tn_gemm_fp8        : D[M,N] = A[M,K]·B[N,K]ᵀ (+R), bf16 or fp32 D.
+ *   tn_gemm_swiglu_fp8 : G, U, H of tn_gemm_swiglu_bf16 from X[M,K] and Wg, Wu [N,K].
+ *   tn_gemm_dswiglu_fp8: dG, dU of tn_gemm_dswiglu_bf16; W = the transposed down_proj weight [N = ffn, K = d].
+ *   tn_gemm_qkv_fp8    : modes of tn_gemm_qkv_bf16.  Mode 1: B_i = [N, s_i] column blocks of Wᵀ = [Wq;Wk;Wv]ᵀ
+ *                        (row stride ldb).  Mode 2: A = the transposed gradient [s0+s1+s2, K], B0 = the transposed
+ *                        layer input [N, K]. */
+int tn_gemm_fp8(const void* A, int64_t lda, int a_e5m2, const void* B, int64_t ldb, void* D, int64_t ldd, int d_f32,
+                const void* R, int64_t ldr, int M, int N, int K, const float* inv_sa, const float* inv_sb,
+                tn_stream_t stream);
+int tn_gemm_swiglu_fp8(const void* X, int64_t ldx, int x_e5m2, const void* Wg, const void* Wu, int64_t ldw, void* G,
+                       void* U, void* H, int64_t ldh, int M, int N, int K, const float* inv_sx, const float* inv_sw,
+                       tn_stream_t stream);
+int tn_gemm_dswiglu_fp8(const void* dY, int64_t lddy, int dy_e5m2, const void* W, int64_t ldw, const void* G,
+                        const void* U, int64_t ldgu, void* dG, void* dU, int64_t lddg, int M, int N, int K,
+                        const float* inv_sa, const float* inv_sb, tn_stream_t stream);
+int tn_gemm_qkv_fp8(int mode, const void* A, int64_t lda, int a_e5m2, const void* B0, const void* B1, const void* B2,
+                    int64_t ldb, void* D0, void* D1, void* D2, int64_t ldd, int d_f32, int s0, int s1, int s2, int M,
+                    int N, int K, const void* rope_cos, const void* rope_sin, const float* inv_sa, const float* inv_sb,
+                    tn_stream_t stream);
+
+/* Dynamic per-tensor FP8 scaling (bf16 [rows, cols] views, rows and cols multiples of 16):
+ *   tn_fp8_amax_bf16: *amax = max(*amax, max|x|) (atomic; the caller zeroes it; several calls share one amax).
+ *   tn_fp8_cast_bf16: s = fmax / max(*amax, 1e-12) (fmax 448 e4m3, 57344 e5m2 with e5m2 = 1); out = sat_rne(x·s)
+ *                     row-major [rows, cols] and/or out_t = its transpose [cols, rows] (either may be NULL); *inv_scale
+ *                     = 1/s if inv_scale is not NULL.  NaN stays NaN. */
+int tn_fp8_amax_bf16(const void* x, int64_t ldx, int64_t rows, int64_t cols, float* amax, tn_stream_t stream);
+int tn_fp8_cast_bf16(const void* x, int64_t ldx, int64_t rows, int64_t cols, int e5m2, const float* amax, void* out,
+                     int64_t ld_out, void* out_t, int64_t ld_out_t, float* inv_scale, tn_stream_t stream);
+
 /* SwiGLU backward (elementwise): dG = dH⊙U⊙silu'(G), dU = dH⊙silu(G).  bf16 [M,N] contiguous rows (ld). */
 int tn_swiglu_bwd_bf16(const void* G, const void* U, const void* dH, void* dG, void* dU, int64_t rows, int64_t cols,
                        int64_t ld, tn_stream_t stream);

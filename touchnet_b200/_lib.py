@@ -29,6 +29,13 @@ _SIGNATURES = {
     "tn_gemm_dswiglu_bf16": [_vp, _i64, _vp, _i64, _vp, _vp, _i64, _vp, _vp, _i64, _i, _i, _i, _vp],
     "tn_gemm_qkv_bf16": [_i, _vp, _i64, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _i64, _i, _i, _i, _i, _i, _i, _i, _vp, _vp,
                          _vp],
+    "tn_gemm_fp8": [_vp, _i64, _i, _vp, _i64, _vp, _i64, _i, _vp, _i64, _i, _i, _i, _vp, _vp, _vp],
+    "tn_gemm_swiglu_fp8": [_vp, _i64, _i, _vp, _vp, _i64, _vp, _vp, _vp, _i64, _i, _i, _i, _vp, _vp, _vp],
+    "tn_gemm_dswiglu_fp8": [_vp, _i64, _i, _vp, _i64, _vp, _vp, _i64, _vp, _vp, _i64, _i, _i, _i, _vp, _vp, _vp],
+    "tn_gemm_qkv_fp8": [_i, _vp, _i64, _i, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _i64, _i, _i, _i, _i, _i, _i, _i, _vp, _vp,
+                        _vp, _vp, _vp],
+    "tn_fp8_amax_bf16": [_vp, _i64, _i64, _i64, _vp, _vp],
+    "tn_fp8_cast_bf16": [_vp, _i64, _i64, _i64, _i, _vp, _vp, _i64, _vp, _i64, _vp, _vp],
     "tn_swiglu_bwd_bf16": [_vp, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _vp],
     "tn_rmsnorm_fwd_bf16": [_vp, _vp, _vp, _i, _vp, _vp, _vp, _i64, _i, _f, _vp],
     "tn_rmsnorm_bwd_bf16": [_vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _i, _vp, _i64, _i, _vp],

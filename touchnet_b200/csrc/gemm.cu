@@ -17,6 +17,12 @@
 // forward, dgrad and wgrad all run on the tensors where they lie: no transposes, no copies.  Epilogues: D = acc (+R) in
 // bf16 or fp32, SwiGLU (gate and up halves of one tile), SwiGLU backward on the dH accumulator, RoPE on the q/k columns of
 // the fused QKV projection.  Each output element sums its k-blocks in the same order at either tile width.
+// FP8 (OP != 0): the same kernel on 8-bit operands, both K-major (8-bit wgmma has no transpose bits).  A stage holds
+// 128 k (the same 128-byte swizzled rows, stage bytes and stage count) and takes four wgmma k32 steps; the epilogue
+// starts by multiplying the accumulator with the two per-tensor inverse scales read from device memory.  Forward
+// (e4m3 A) accumulates in the wgmma accumulator alone; dgrad and wgrad (e5m2 A) add each stage's partial sum into a
+// separate fp32 accumulator, because the 8-bit MMAs accumulate with reduced precision.  That doubles the accumulator
+// registers, so the promoted form runs on the 128-wide tile only.
 #include <stdio.h>
 #include <stdlib.h>
 
@@ -68,6 +74,9 @@ struct GemmParams {
   const bf16* aux_g;
   const bf16* aux_u;
   int64_t ld_gu;
+  // FP8: 1/s of the A and B operands (device floats written by tn_fp8_cast_bf16)
+  const float* inv_sa;
+  const float* inv_sb;
 };
 
 // Operand and output tensor maps.  d[]: EPI 0/2 the output (d_seg: one map per segment), EPI 1 H / G / U, EPI 3 dG / dU;
@@ -86,9 +95,13 @@ __device__ __forceinline__ void decode_tile(int tile, int num_m, int num_n, int 
   n_blk = r / gsize;
 }
 
-template <int BN, bool A_MN, bool B_MN, int EPI>
+// OP: operand type and accumulation.  0 = bf16;  1 = e4m3 A, e4m3 B, accumulated in the wgmma accumulator (forward);
+//     2 = e5m2 A, e4m3 B, stage partial sums promoted into a separate fp32 accumulator (dgrad / wgrad, BN 128 only)
+template <int BN, bool A_MN, bool B_MN, int EPI, int OP = 0>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_kernel(const __grid_constant__ GemmMaps tm, const GemmParams p) {
+  static_assert(OP == 0 || (!A_MN && !B_MN), "8-bit operands are K-major");
+  static_assert(OP != 2 || BN == 128, "the promoted accumulator fits the 128-wide tile only");
   using C = TileCfg<BN>;
   constexpr int STAGES = C::STAGES;
   extern __shared__ uint8_t smem_raw[];
@@ -138,7 +151,7 @@ gemm_kernel(const __grid_constant__ GemmMaps tm, const GemmParams p) {
           mbar_arrive_expect_tx(&full_bar[stage], C::STAGE_BYTES);
           uint8_t* a_dst = sA + stage * A_BYTES;
           uint8_t* b_dst = sB + stage * C::B_BYTES;
-          const int k0 = kb * BK;
+          const int k0 = kb * (OP ? 2 * BK : BK);   // k per stage: 128-byte operand rows either way
           int kb0 = k0;   // k coordinate inside the selected B segment
           if (p.b_seg == 2) {
             const int sg = (k0 >= p.off1) + (k0 >= p.off2);
@@ -246,16 +259,35 @@ gemm_kernel(const __grid_constant__ GemmMaps tm, const GemmParams p) {
       const uint32_t a_addr = smem_u32(sA + stage * A_BYTES) + uint32_t(c) * 8192u;
       const uint32_t b_addr = smem_u32(sB + stage * C::B_BYTES);
       wgmma_fence();
+      if constexpr (OP == 2) {
+        float part[BN / 2];                      // this stage's partial sum
 #pragma unroll
-      for (int k = 0; k < BK / 16; ++k) {
-        const uint64_t da = A_MN ? make_sdesc_sw128(a_addr + k * 2048, 8192, 1024) : make_sdesc_sw128(a_addr + k * 32, 16, 1024);
-        const uint64_t db = B_MN ? make_sdesc_sw128(b_addr + k * 2048, 8192, 1024) : make_sdesc_sw128(b_addr + k * 32, 16, 1024);
-        if constexpr (BN == 256) wgmma_m64n256<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, 1u);
-        else wgmma_m64n128<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, 1u);
+        for (int k = 0; k < 4; ++k)
+          wgmma_fp8_m64n128<true>(part, make_sdesc_sw128(a_addr + k * 32, 16, 1024),
+                                  make_sdesc_sw128(b_addr + k * 32, 16, 1024), k > 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(part);
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];
+      } else {
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k) {
+          const uint64_t da = A_MN ? make_sdesc_sw128(a_addr + k * 2048, 8192, 1024) : make_sdesc_sw128(a_addr + k * 32, 16, 1024);
+          const uint64_t db = B_MN ? make_sdesc_sw128(b_addr + k * 2048, 8192, 1024) : make_sdesc_sw128(b_addr + k * 32, 16, 1024);
+          if constexpr (OP == 1) {
+            if constexpr (BN == 256) wgmma_fp8_m64n256<false>(acc, da, db, 1u);
+            else wgmma_fp8_m64n128<false>(acc, da, db, 1u);
+          } else if constexpr (BN == 256) {
+            wgmma_m64n256<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, 1u);
+          } else {
+            wgmma_m64n128<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, 1u);
+          }
+        }
+        wgmma_commit();
+        wgmma_wait<1>();                         // the previous k-block's MMAs have retired: its slot can be refilled
+        wgmma_fence_regs(acc);
       }
-      wgmma_commit();
-      wgmma_wait<1>();                           // the previous k-block's MMAs have retired: its slot can be refilled
-      wgmma_fence_regs(acc);
       if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
       prev = stage;
       if (++stage == STAGES) { stage = 0; phase ^= 1; }
@@ -263,6 +295,11 @@ gemm_kernel(const __grid_constant__ GemmMaps tm, const GemmParams p) {
     wgmma_wait<0>();
     wgmma_fence_regs(acc);
     if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+    if constexpr (OP != 0) {   // dequantise: acc · (1/s_a)·(1/s_b), ahead of every epilogue
+      const float sc = *p.inv_sa * *p.inv_sb;
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] *= sc;
+    }
 
     // ---------------- epilogue: registers -> swizzled staging (-> coalesced pass) -> TMA store ----------------
     const int m0 = m_blk * BM;
@@ -455,9 +492,9 @@ gemm_kernel(const __grid_constant__ GemmMaps tm, const GemmParams p) {
   if (t == 0) tma_store_wait<0>();   // staging must stay valid until the last stores have read it
 }
 
-template <int BN, bool A_MN, bool B_MN, int EPI>
+template <int BN, bool A_MN, bool B_MN, int EPI, int OP = 0>
 static int launch_gemm(const GemmMaps& tm, const GemmParams& p, cudaStream_t stream) {
-  auto kern = gemm_kernel<BN, A_MN, B_MN, EPI>;
+  auto kern = gemm_kernel<BN, A_MN, B_MN, EPI, OP>;
   constexpr int smem = TileCfg<BN>::SMEM;
   static bool configured = false;  // per instantiation
   if (!configured) {
@@ -490,12 +527,12 @@ static int pick_bn(int M, int N, int out_div) {
   return double(w_wide) * kWideTileCost <= double(w_narrow) ? 256 : 128;
 }
 
-static GemmParams base_params(int M, int N, int K, int tile_n) {
+static GemmParams base_params(int M, int N, int K, int tile_n, int kb = BK) {
   GemmParams p{};
   p.M = M; p.N = N; p.K = K;
   p.num_m = (M + BM - 1) / BM;
   p.num_n = (N + tile_n - 1) / tile_n;
-  p.num_k = (K + BK - 1) / BK;
+  p.num_k = (K + kb - 1) / kb;
   p.group = gemm_group();
   // L2 policy: inside a raster group the `group` A strips are re-read by every wave, a B strip is consumed within
   // about one wave -> A evict-last, B evict-first (tn_set_gemm_l2_hints; default off)
@@ -509,6 +546,29 @@ static int map_operand(CUtensorMap* m, const void* ptr, int mn, uint64_t rows, u
   if (!mn) return encode_tmap_2d(m, ptr, 2, K, rows, uint64_t(ld) * 2, 64, box_rows, true);
   return encode_tmap_2d(m, ptr, 2, rows, K, uint64_t(ld) * 2, 64, 64, true);
 }
+
+// K-major 8-bit operand [rows, K] (K contiguous, ld bytes) -> box {128 k, box_rows}: the same 128-byte rows
+static int map_operand_fp8(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t K, int64_t ld, uint32_t box_rows) {
+  return encode_tmap_2d(m, ptr, 1, K, rows, uint64_t(ld), 128, box_rows, true);
+}
+
+// FP8 launches: the operand type of A selects the accumulation (see gemm_kernel's OP), the promoted form the 128 tile
+static int fp8_bn(int a_e5m2, int M, int N, int out_div) { return a_e5m2 ? 128 : pick_bn(M, N, out_div); }
+
+template <int EPI>
+static int launch_fp8(int a_e5m2, int bn, const GemmMaps& tm, const GemmParams& p, cudaStream_t stream) {
+  if (a_e5m2) return launch_gemm<128, false, false, EPI, 2>(tm, p, stream);
+  return bn == 256 ? launch_gemm<256, false, false, EPI, 1>(tm, p, stream)
+                   : launch_gemm<128, false, false, EPI, 1>(tm, p, stream);
+}
+
+static GemmParams fp8_params(int M, int N, int K, int tile_n, const float* inv_sa, const float* inv_sb) {
+  GemmParams p = base_params(M, N, K, tile_n, 2 * BK);
+  p.inv_sa = inv_sa; p.inv_sb = inv_sb;
+  return p;
+}
+
+static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 // output [rows, cols] (row stride ld elements) -> box of one staging sub-tile: 64 rows x (64 bf16 | 32 fp32) columns
 static int map_output(CUtensorMap* m, const void* ptr, int f32, uint64_t rows, uint64_t cols, int64_t ld) {
@@ -664,3 +724,147 @@ extern "C" int tn_gemm_qkv_bf16(int mode, const void* A, int64_t lda, const void
     if ((rc = map_output(&tm.d[i], Ds[i], d_f32, uint64_t(seg[i]), uint64_t(N), ldd))) return rc;
   return d_f32 ? launch_gemm<true, true, 2>(bn, tm, p, stream) : launch_gemm<true, true, 0>(bn, tm, p, stream);
 }
+
+// ---------------------------------------------------------------------------------------------------------------
+// FP8 twins of the entry points above: K-major 8-bit operands (A e4m3, or e5m2 with a_e5m2; B e4m3), 1/s_a and 1/s_b
+// read from device memory (tn_fp8_cast_bf16), outputs and epilogues as in the bf16 entry points.  Every dimension and
+// leading dimension is a multiple of 16 (TMA rows of 8-bit elements are 16-byte aligned).
+// ---------------------------------------------------------------------------------------------------------------
+#define TN_FP8_REQUIRE_COMMON(name, A, lda, B, ldb, inv_sa, inv_sb, M, N, K)                                          \
+  TN_REQUIRE(A && B && inv_sa && inv_sb, name ": null pointer");                                                    \
+  TN_REQUIRE(M > 0 && N > 0 && K > 0 && M % 16 == 0 && N % 16 == 0 && K % 16 == 0,                                   \
+             name ": M=%d N=%d K=%d must be positive multiples of 16", M, N, K);                                      \
+  TN_REQUIRE(lda % 16 == 0 && ldb % 16 == 0 && aligned16(A) && aligned16(B),                                        \
+             name ": A and B must be 16 B aligned with leading dims that are multiples of 16")
+
+extern "C" int tn_gemm_fp8(const void* A, int64_t lda, int a_e5m2, const void* B, int64_t ldb, void* D, int64_t ldd,
+                           int d_f32, const void* R, int64_t ldr, int M, int N, int K, const float* inv_sa,
+                           const float* inv_sb, tn_stream_t stream_) {
+  clear_error();
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  TN_REQUIRE(D, "tn_gemm_fp8: null pointer");
+  TN_FP8_REQUIRE_COMMON("tn_gemm_fp8", A, lda, B, ldb, inv_sa, inv_sb, M, N, K);
+  TN_REQUIRE(ldd % (d_f32 ? 4 : 8) == 0 && (!R || ldr % (d_f32 ? 4 : 8) == 0), "tn_gemm_fp8: ldd/ldr alignment");
+  TN_REQUIRE(aligned16(D) && (!R || aligned16(R)), "tn_gemm_fp8: D/R must be 16 B aligned");
+  const int bn = fp8_bn(a_e5m2, M, N, 1);
+  GemmParams p = fp8_params(M, N, K, bn, inv_sa, inv_sb);
+  p.R = R; p.ldr = ldr;
+  GemmMaps tm;
+  int rc;
+  if ((rc = map_operand_fp8(&tm.a, A, uint64_t(M), uint64_t(K), lda, BM))) return rc;
+  if ((rc = map_operand_fp8(&tm.b[0], B, uint64_t(N), uint64_t(K), ldb, bn))) return rc;
+  if ((rc = map_output(&tm.d[0], D, d_f32, uint64_t(M), uint64_t(N), ldd))) return rc;
+  tm.b[1] = tm.b[2] = tm.b[0];
+  tm.d[1] = tm.d[2] = tm.d[0];
+  return d_f32 ? launch_fp8<2>(a_e5m2, bn, tm, p, stream) : launch_fp8<0>(a_e5m2, bn, tm, p, stream);
+}
+
+extern "C" int tn_gemm_swiglu_fp8(const void* X, int64_t ldx, int x_e5m2, const void* Wg, const void* Wu, int64_t ldw,
+                                  void* G, void* U, void* H, int64_t ldh, int M, int N, int K, const float* inv_sx,
+                                  const float* inv_sw, tn_stream_t stream_) {
+  clear_error();
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  TN_REQUIRE(Wu && H, "tn_gemm_swiglu_fp8: null pointer");
+  TN_FP8_REQUIRE_COMMON("tn_gemm_swiglu_fp8", X, ldx, Wg, ldw, inv_sx, inv_sw, M, N, K);
+  TN_REQUIRE(ldh % 8 == 0 && aligned16(Wu), "tn_gemm_swiglu_fp8: ldh must be a multiple of 8, Wu 16 B aligned");
+  TN_REQUIRE(aligned16(H) && (!G || aligned16(G)) && (!U || aligned16(U)), "tn_gemm_swiglu_fp8: outputs must be 16 B aligned");
+  const int bn = fp8_bn(x_e5m2, M, N, 2);
+  GemmParams p = fp8_params(M, N, K, bn / 2, inv_sx, inv_sw);
+  p.has_g = G != nullptr; p.has_u = U != nullptr;
+  GemmMaps tm;
+  int rc;
+  if ((rc = map_operand_fp8(&tm.a, X, uint64_t(M), uint64_t(K), ldx, BM))) return rc;
+  if ((rc = map_operand_fp8(&tm.b[0], Wg, uint64_t(N), uint64_t(K), ldw, bn / 2))) return rc;
+  if ((rc = map_operand_fp8(&tm.b[1], Wu, uint64_t(N), uint64_t(K), ldw, bn / 2))) return rc;
+  tm.b[2] = tm.b[1];
+  if ((rc = map_output(&tm.d[0], H, 0, uint64_t(M), uint64_t(N), ldh))) return rc;
+  tm.d[1] = tm.d[2] = tm.d[0];
+  if (G && (rc = map_output(&tm.d[1], G, 0, uint64_t(M), uint64_t(N), ldh))) return rc;
+  if (U && (rc = map_output(&tm.d[2], U, 0, uint64_t(M), uint64_t(N), ldh))) return rc;
+  return launch_fp8<1>(x_e5m2, bn, tm, p, stream);
+}
+
+// W is the K-major transposed copy of down_proj.weight: [N = ffn, K = d]
+extern "C" int tn_gemm_dswiglu_fp8(const void* dY, int64_t lddy, int dy_e5m2, const void* W, int64_t ldw, const void* G,
+                                   const void* U, int64_t ldgu, void* dG, void* dU, int64_t lddg, int M, int N, int K,
+                                   const float* inv_sa, const float* inv_sb, tn_stream_t stream_) {
+  clear_error();
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  TN_REQUIRE(G && U && dG && dU, "tn_gemm_dswiglu_fp8: null pointer");
+  TN_FP8_REQUIRE_COMMON("tn_gemm_dswiglu_fp8", dY, lddy, W, ldw, inv_sa, inv_sb, M, N, K);
+  TN_REQUIRE(M >= 256 && N >= 256, "tn_gemm_dswiglu_fp8: needs M, N >= 256");
+  TN_REQUIRE(ldgu % 8 == 0 && lddg % 8 == 0, "tn_gemm_dswiglu_fp8: ldgu and lddg must be multiples of 8");
+  TN_REQUIRE(aligned16(G) && aligned16(U) && aligned16(dG) && aligned16(dU),
+             "tn_gemm_dswiglu_fp8: G, U, dG, dU must be 16 B aligned");
+  const int bn = fp8_bn(dy_e5m2, M, N, 1);
+  GemmParams p = fp8_params(M, N, K, bn, inv_sa, inv_sb);
+  p.aux_g = static_cast<const bf16*>(G); p.aux_u = static_cast<const bf16*>(U); p.ld_gu = ldgu;
+  GemmMaps tm;
+  int rc;
+  if ((rc = map_operand_fp8(&tm.a, dY, uint64_t(M), uint64_t(K), lddy, BM))) return rc;
+  if ((rc = map_operand_fp8(&tm.b[0], W, uint64_t(N), uint64_t(K), ldw, bn))) return rc;
+  tm.b[1] = tm.b[2] = tm.b[0];
+  if ((rc = map_output(&tm.d[0], dG, 0, uint64_t(M), uint64_t(N), lddg))) return rc;
+  if ((rc = map_output(&tm.d[1], dU, 0, uint64_t(M), uint64_t(N), lddg))) return rc;
+  tm.d[2] = tm.d[1];
+  return launch_fp8<3>(dy_e5m2, bn, tm, p, stream);
+}
+
+// Modes as tn_gemm_qkv_bf16, all operands K-major: 1 = dgrad with B_i the [N, s_i] column blocks of Wᵀ (row stride
+// ldb), 2 = wgrad with A = the transposed gradient [s0+s1+s2, K] and B0 = the transposed layer input [N, K].
+extern "C" int tn_gemm_qkv_fp8(int mode, const void* A, int64_t lda, int a_e5m2, const void* B0, const void* B1,
+                               const void* B2, int64_t ldb, void* D0, void* D1, void* D2, int64_t ldd, int d_f32, int s0,
+                               int s1, int s2, int M, int N, int K, const void* rope_cos, const void* rope_sin,
+                               const float* inv_sa, const float* inv_sb, tn_stream_t stream_) {
+  clear_error();
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  TN_REQUIRE(D0, "tn_gemm_qkv_fp8: null pointer");
+  TN_FP8_REQUIRE_COMMON("tn_gemm_qkv_fp8", A, lda, B0, ldb, inv_sa, inv_sb, M, N, K);
+  TN_REQUIRE(mode >= 0 && mode <= 2, "tn_gemm_qkv_fp8: mode must be 0 (forward), 1 (dgrad) or 2 (wgrad)");
+  TN_REQUIRE(s0 > 0 && s1 > 0 && s2 > 0 && s0 % 256 == 0 && s1 % 256 == 0 && s2 % 256 == 0,
+             "tn_gemm_qkv_fp8: segment sizes (%d,%d,%d) must be positive multiples of 256", s0, s1, s2);
+  const int tot = s0 + s1 + s2;
+  TN_REQUIRE((mode == 0 && N == tot) || (mode == 1 && K == tot) || (mode == 2 && M == tot),
+             "tn_gemm_qkv_fp8: segments do not add up to the segmented dimension");
+  TN_REQUIRE(M >= 256 && N >= 256 && ldd % (d_f32 ? 4 : 8) == 0,
+             "tn_gemm_qkv_fp8: needs M,N >= 256 and 16-byte aligned leading dimensions");
+  TN_REQUIRE(mode == 2 || (B1 && B2 && aligned16(B1) && aligned16(B2)), "tn_gemm_qkv_fp8: B1/B2 required, 16 B aligned");
+  TN_REQUIRE(mode != 2 || (D1 && D2), "tn_gemm_qkv_fp8: D1/D2 required for wgrad");
+  TN_REQUIRE((rope_cos == nullptr) == (rope_sin == nullptr), "tn_gemm_qkv_fp8: cos and sin tables come in pairs");
+  TN_REQUIRE(rope_cos == nullptr || mode == 0, "tn_gemm_qkv_fp8: fused RoPE exists for the forward projection only");
+  const void* Bs[3] = {B0, B1, B2};
+  const int seg[3] = {s0, s1, s2};
+  const int bn = fp8_bn(a_e5m2, M, N, 1);
+  GemmParams p = fp8_params(M, N, K, bn, inv_sa, inv_sb);
+  p.off1 = s0; p.off2 = s0 + s1;
+  GemmMaps tm;
+  int rc;
+  if ((rc = map_operand_fp8(&tm.a, A, uint64_t(M), uint64_t(K), lda, BM))) return rc;
+  if (mode == 2) {
+    p.d_seg = 1;
+    void* Ds[3] = {D0, D1, D2};
+    if ((rc = map_operand_fp8(&tm.b[0], B0, uint64_t(N), uint64_t(K), ldb, bn))) return rc;
+    tm.b[1] = tm.b[2] = tm.b[0];
+    for (int i = 0; i < 3; ++i)
+      if ((rc = map_output(&tm.d[i], Ds[i], d_f32, uint64_t(seg[i]), uint64_t(N), ldd))) return rc;
+    return d_f32 ? launch_fp8<2>(a_e5m2, bn, tm, p, stream) : launch_fp8<0>(a_e5m2, bn, tm, p, stream);
+  }
+  if (mode == 0) {
+    if (rope_cos) {
+      p.rope_cos = static_cast<const bf16*>(rope_cos); p.rope_sin = static_cast<const bf16*>(rope_sin);
+      p.rope_end = s0 + s1;
+    }
+    p.b_seg = 1;
+    for (int i = 0; i < 3; ++i)
+      if ((rc = map_operand_fp8(&tm.b[i], Bs[i], uint64_t(seg[i]), uint64_t(K), ldb, bn))) return rc;
+  } else {
+    p.b_seg = 2;
+    for (int i = 0; i < 3; ++i)
+      if ((rc = map_operand_fp8(&tm.b[i], Bs[i], uint64_t(N), uint64_t(seg[i]), ldb, bn))) return rc;
+  }
+  TN_REQUIRE(!d_f32, "tn_gemm_qkv_fp8: modes 0 and 1 write bf16");
+  if ((rc = map_output(&tm.d[0], D0, 0, uint64_t(M), uint64_t(N), ldd))) return rc;
+  tm.d[1] = tm.d[2] = tm.d[0];
+  return launch_fp8<0>(a_e5m2, bn, tm, p, stream);
+}
+#undef TN_FP8_REQUIRE_COMMON

@@ -59,7 +59,9 @@ static int encode_nd(CUtensorMap* out, const void* ptr, int elem_bytes, int rank
       return fail(TN_ERR_ARG, "TMA stride %d = %llu bytes is not a multiple of 16", i,
                   (unsigned long long)strides_bytes[i]);
   }
-  CUtensorMapDataType dt = elem_bytes == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+  CUtensorMapDataType dt = elem_bytes == 1   ? CU_TENSOR_MAP_DATA_TYPE_UINT8
+                           : elem_bytes == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                             : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
   CUresult r = enc(out, dt, rank, const_cast<void*>(ptr), gdim, gstr, gbox, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                    swizzle128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);

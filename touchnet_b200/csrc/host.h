@@ -27,7 +27,7 @@ enum { TN_OK = 0, TN_ERR_ARG = 1, TN_ERR_CUDA = 2, TN_ERR_UNSUPPORTED = 3 };
   } while (0)
 
 // TMA descriptor encoders (driver entry point resolved lazily through the runtime; no -lcuda link).
-// elem_bytes: 2 (bf16) or 4 (f32).  Strides in bytes (must be multiples of 16).  SWIZZLE_128B iff swizzle128.
+// elem_bytes: 1 (FP8, as uint8), 2 (bf16) or 4 (f32).  Strides in bytes (must be multiples of 16).  SWIZZLE_128B iff swizzle128.
 int encode_tmap_2d(CUtensorMap* out, const void* ptr, int elem_bytes, uint64_t dim0, uint64_t dim1,
                    uint64_t stride1_bytes, uint32_t box0, uint32_t box1, bool swizzle128);
 int encode_tmap_3d(CUtensorMap* out, const void* ptr, int elem_bytes, uint64_t dim0, uint64_t dim1, uint64_t dim2,

@@ -151,14 +151,14 @@ class B200DecoderLayer(nn.Module):
         self.input_layernorm = B200RMSNorm(config.hidden_size, eps)
         self.post_attention_layernorm = B200RMSNorm(config.hidden_size, eps)
 
-    def forward(self, hidden_states, cos, sin, plan):
+    def forward(self, hidden_states, cos, sin, plan, fp8: bool = False):
         a, m = self.self_attn, self.mlp
         if plan.tp is None:
             return ops.decoder_layer(
                 hidden_states, self.input_layernorm.weight, a.q_proj.weight, a.k_proj.weight, a.v_proj.weight,
                 a.q_proj.bias, a.k_proj.bias, a.v_proj.bias, a.o_proj.weight, self.post_attention_layernorm.weight,
                 m.gate_proj.weight, m.up_proj.weight, m.down_proj.weight, cos, sin, plan, a.num_heads,
-                a.num_key_value_heads, self.input_layernorm.variance_epsilon, a.head_dim)
+                a.num_key_value_heads, self.input_layernorm.variance_epsilon, a.head_dim, fp8)
         # tensor parallel (tensor_parallel.py): this rank's weight shards, H/tp and KV/tp heads
         from .tensor_parallel import local
         wq, wk = local(a.q_proj.weight), local(a.k_proj.weight)
@@ -167,7 +167,7 @@ class B200DecoderLayer(nn.Module):
             local(a.q_proj.bias), local(a.k_proj.bias), local(a.v_proj.bias), local(a.o_proj.weight),
             local(self.post_attention_layernorm.weight), local(m.gate_proj.weight), local(m.up_proj.weight),
             local(m.down_proj.weight), cos, sin, plan, wq.shape[0] // a.head_dim, wk.shape[0] // a.head_dim,
-            self.input_layernorm.variance_epsilon)
+            self.input_layernorm.variance_epsilon, fp8=fp8)
 
 
 class B200LlamaModel(nn.Module):
@@ -182,6 +182,9 @@ class B200LlamaModel(nn.Module):
         self.layers = nn.ModuleList([B200DecoderLayer(config, i) for i in range(config.num_hidden_layers)])
         self.norm = B200RMSNorm(config.hidden_size, _cfg(config, "rms_norm_eps", 1e-6))
         self.rotary_emb = B200RotaryEmbedding(config)
+        # FP8 projections in every decoder block (ops.block_forward); cached decoding stays bf16.  A plain attribute:
+        # no parameter or buffer, so state dicts do not change
+        self.float8_training = bool(_cfg(config, "float8_training", False))
         hd = _cfg(config, "head_dim", config.hidden_size // config.num_attention_heads)
         if hd > 128 or hd % 8:
             raise TouchNetB200Error(f"touchnet_b200 attention kernels are built for head_dim 128 (smaller multiples of 8 run "
@@ -222,7 +225,7 @@ class B200LlamaModel(nn.Module):
         if x.dtype != torch.bfloat16:
             x = x.to(torch.bfloat16)
         for layer in self.layers:
-            x = layer(x, cos, sin, plan)
+            x = layer(x, cos, sin, plan, self.float8_training)
         return self.norm(x)
 
 
@@ -291,13 +294,23 @@ class B200LlamaForCausalLM(nn.Module):
     def __init__(self, config):
         super().__init__()
         self.config = config
-        self.model = B200LlamaModel(config)
+        self.model = B200LlamaModel(config)       # reads the config key `float8_training`
         self.vocab_size = config.vocab_size
         self.lm_head = nn.Linear(config.hidden_size, config.vocab_size, bias=False)
         if _cfg(config, "tie_word_embeddings", False):
             self.lm_head.weight = self.model.embed_tokens.weight
         else:
             self._tied_weights_keys = None
+
+    @property
+    def float8_training(self) -> bool:
+        """FP8 (torchao tensorwise recipe) for the q/k/v/o/gate/up/down projections of every decoder block, forward and
+        backward; lm_head, attention, norms and cached decoding stay bf16.  Set from the config key `float8_training`."""
+        return self.model.float8_training
+
+    @float8_training.setter
+    def float8_training(self, v: bool):
+        self.model.float8_training = bool(v)
 
     # -- HF surface the reference touches -------------------------------------------------------------------
     def get_input_embeddings(self):
@@ -426,6 +439,8 @@ class B200TouchAudioForCausalLM(nn.Module):
         self.register_buffer("_nan_flag", torch.zeros(1, dtype=torch.int32), persistent=False)
         # lm_head.weight belongs to the FSDP2 ROOT group when this wrapper is the root: the inner model asks it
         object.__setattr__(self.language_model, "_tn_fsdp_root", self)
+        if getattr(config, "float8_training", None) is not None:   # the top-level key of the model JSON wins
+            self.float8_training = config.float8_training
 
     @property
     def fused_linear_ce(self) -> bool:
@@ -434,6 +449,14 @@ class B200TouchAudioForCausalLM(nn.Module):
     @fused_linear_ce.setter
     def fused_linear_ce(self, v: bool):
         self.language_model.fused_linear_ce = bool(v)
+
+    @property
+    def float8_training(self) -> bool:
+        return self.language_model.float8_training
+
+    @float8_training.setter
+    def float8_training(self, v: bool):
+        self.language_model.float8_training = bool(v)
 
     @property
     def model(self):  # the reference's llama post_init / get_num_params reach `model.model.*`

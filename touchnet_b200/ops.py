@@ -258,6 +258,152 @@ def gemm_dswiglu(dy: torch.Tensor, wd: torch.Tensor, g: torch.Tensor, u: torch.T
     return dg, du
 
 
+# ---------------------------------------------------------------------------------------------------------------
+# FP8 (torchao's tensorwise recipe): dynamic per-tensor scales that never leave the device, K-major 8-bit operands
+# ---------------------------------------------------------------------------------------------------------------
+F8E4M3, F8E5M2 = torch.float8_e4m3fn, torch.float8_e5m2
+
+
+def fp8_amax(x: torch.Tensor, amax: torch.Tensor) -> None:
+    """amax = max(amax, max|x|) over a bf16 [rows, cols] view; `amax` is a device float the caller zeroed."""
+    _chk(x, "x", BF16)
+    _lib.call("tn_fp8_amax_bf16", x.data_ptr(), x.stride(0), x.shape[0], x.shape[1], amax.data_ptr(), _st())
+
+
+def fp8_cast(x: torch.Tensor, amax: torch.Tensor, e5m2: bool, row: bool = True, t: bool = True, inv=None, out=None,
+             out_t=None):
+    """sat_rne(x · s) with s = fmax / max(amax, 1e-12): the row-major copy [rows, cols] (row=True) and / or the
+    transposed copy [cols, rows] (t=True), e5m2 or e4m3, from one read of bf16 x; 1/s goes to `inv` if given.
+    Returns (row-major or None, transposed or None)."""
+    _chk(x, "x", BF16)
+    rows, cols = x.shape
+    dt = F8E5M2 if e5m2 else F8E4M3
+    if row and out is None:
+        out = torch.empty((rows, cols), dtype=dt, device=x.device)
+    if t and out_t is None:
+        out_t = torch.empty((cols, rows), dtype=dt, device=x.device)
+    _lib.call("tn_fp8_cast_bf16", x.data_ptr(), x.stride(0), rows, cols, int(e5m2), amax.data_ptr(), _lib.ptr(out),
+              0 if out is None else out.stride(0), _lib.ptr(out_t), 0 if out_t is None else out_t.stride(0),
+              _lib.ptr(inv), _st())
+    return out, out_t
+
+
+def _fp8_operands(a: torch.Tensor, b: torch.Tensor) -> int:
+    """Checks the operand types of an FP8 GEMM; returns 1 if A is e5m2 (a gradient: promoted accumulation)."""
+    if b.dtype != F8E4M3:
+        raise _lib.TouchNetB200Error(f"the B operand of an FP8 GEMM must be float8_e4m3fn, got {b.dtype} (e5m2 B is not supported)")
+    if a.dtype not in (F8E4M3, F8E5M2):
+        raise _lib.TouchNetB200Error(f"the A operand of an FP8 GEMM must be float8_e4m3fn or float8_e5m2, got {a.dtype}")
+    _chk(a, "a"); _chk(b, "b")
+    assert a.dim() == 2 and b.dim() == 2 and a.stride(1) == 1 and b.stride(1) == 1
+    return int(a.dtype == F8E5M2)
+
+
+def gemm_fp8(a, b, inv_a, inv_b, *, out_f32: bool = False, residual=None, out=None):
+    """D[M,N] = a[M,K]·b[N,K]ᵀ · inv_a · inv_b (+R): both operands K-major 8-bit, inv_* device floats (1/s)."""
+    a_e5m2 = _fp8_operands(a, b)
+    (M, K), N = a.shape, b.shape[0]
+    assert b.shape[1] == K, (a.shape, b.shape)
+    dt = torch.float32 if out_f32 else BF16
+    if out is None:
+        out = torch.empty((M, N), dtype=dt, device=a.device)
+    _lib.call("tn_gemm_fp8", a.data_ptr(), a.stride(0), a_e5m2, b.data_ptr(), b.stride(0), out.data_ptr(), out.stride(0),
+              int(out_f32), _lib.ptr(residual), 0 if residual is None else residual.stride(0), M, N, K, inv_a.data_ptr(),
+              inv_b.data_ptr(), _st())
+    return out
+
+
+def gemm_swiglu_fp8(x, wg, wu, inv_x, inv_w, need_gu: bool = True):
+    """gemm_swiglu on 8-bit x [M,K] and wg / wu [N,K] (one scale for both weights: they share a tile)."""
+    x_e5m2 = _fp8_operands(x, wg)
+    _fp8_operands(x, wu)
+    M, K = x.shape
+    N = wg.shape[0]
+    assert wg.shape == wu.shape == (N, K) and wg.stride(0) == wu.stride(0)
+    h = torch.empty((M, N), dtype=BF16, device=x.device)
+    g = torch.empty_like(h) if need_gu else None
+    u = torch.empty_like(h) if need_gu else None
+    _lib.call("tn_gemm_swiglu_fp8", x.data_ptr(), x.stride(0), x_e5m2, wg.data_ptr(), wu.data_ptr(), wg.stride(0),
+              _lib.ptr(g), _lib.ptr(u), h.data_ptr(), N, M, N, K, inv_x.data_ptr(), inv_w.data_ptr(), _st())
+    return g, u, h
+
+
+def gemm_dswiglu_fp8(dy, wd_t, g, u, inv_a, inv_b):
+    """(dG, dU) from the down-proj dgrad dH = dy[M,K]·wd_t[N,K]ᵀ (wd_t: the transposed down_proj weight) with the SwiGLU
+    backward in the epilogue; below M, N = 256 or without TN_FUSED_DSWIGLU=1 the plain FP8 GEMM + swiglu_bwd."""
+    dy_e5m2 = _fp8_operands(dy, wd_t)
+    M, K = dy.shape
+    N = wd_t.shape[0]
+    if not (_FUSE_DSWIGLU and M >= 256 and N >= 256 and g.stride(0) == u.stride(0)):
+        return swiglu_bwd(g, u, gemm_fp8(dy, wd_t, inv_a, inv_b))
+    dg = torch.empty_like(g)
+    du = torch.empty_like(u)
+    _lib.call("tn_gemm_dswiglu_fp8", dy.data_ptr(), dy.stride(0), dy_e5m2, wd_t.data_ptr(), wd_t.stride(0), g.data_ptr(),
+              u.data_ptr(), g.stride(0), dg.data_ptr(), du.data_ptr(), dg.stride(0), M, N, K, inv_a.data_ptr(),
+              inv_b.data_ptr(), _st())
+    return dg, du
+
+
+def gemm_qkv_fwd_fp8(x, wq, wk, wv, inv_x, inv_w, rope=None):
+    """gemm_qkv_fwd on 8-bit x [M,K] and wq / wk / wv [n_i, K] (one shared weight scale)."""
+    a_e5m2 = _fp8_operands(x, wq)
+    M, K = x.shape
+    nq, nkv = wq.shape[0], wk.shape[0]
+    out = torch.empty((M, nq + 2 * nkv), dtype=BF16, device=x.device)
+    _lib.call("tn_gemm_qkv_fp8", 0, x.data_ptr(), x.stride(0), a_e5m2, wq.data_ptr(), wk.data_ptr(), wv.data_ptr(),
+              wq.stride(0), out.data_ptr(), None, None, out.stride(0), 0, nq, nkv, nkv, M, nq + 2 * nkv, K,
+              None if rope is None else rope[0].data_ptr(), None if rope is None else rope[1].data_ptr(),
+              inv_x.data_ptr(), inv_w.data_ptr(), _st())
+    return out
+
+
+def gemm_qkv_dgrad_fp8(dqkv, w_t, nq: int, nkv: int, inv_a, inv_b):
+    """dx[M, d] = dqkv[M, nq+2nkv]·w_t[d, nq+2nkv]ᵀ, w_t = [Wq;Wk;Wv]ᵀ, as the K-segmented launch."""
+    a_e5m2 = _fp8_operands(dqkv, w_t)
+    M, Kt = dqkv.shape
+    d = w_t.shape[0]
+    out = torch.empty((M, d), dtype=BF16, device=dqkv.device)
+    _lib.call("tn_gemm_qkv_fp8", 1, dqkv.data_ptr(), dqkv.stride(0), a_e5m2, w_t.data_ptr(), w_t[:, nq:].data_ptr(),
+              w_t[:, nq + nkv:].data_ptr(), w_t.stride(0), out.data_ptr(), None, None, out.stride(0), 0, nq, nkv, nkv,
+              M, d, Kt, None, None, inv_a.data_ptr(), inv_b.data_ptr(), _st())
+    return out
+
+
+def gemm_qkv_wgrad_fp8(dqkv_t, x_t, f32: bool, nq: int, nkv: int, inv_a, inv_b):
+    """(dWq, dWk, dWv) = row blocks of dqkv_t[nq+2nkv, M]·x_t[d, M]ᵀ in one launch (fp32 for fp32 master weights)."""
+    a_e5m2 = _fp8_operands(dqkv_t, x_t)
+    Mt, Mred = dqkv_t.shape
+    d = x_t.shape[0]
+    dt = torch.float32 if f32 else BF16
+    outs = [torch.empty((n, d), dtype=dt, device=x_t.device) for n in (nq, nkv, nkv)]
+    _lib.call("tn_gemm_qkv_fp8", 2, dqkv_t.data_ptr(), dqkv_t.stride(0), a_e5m2, x_t.data_ptr(), None, None,
+              x_t.stride(0), outs[0].data_ptr(), outs[1].data_ptr(), outs[2].data_ptr(), d, int(f32), nq, nkv, nkv, Mt, d,
+              Mred, None, None, inv_a.data_ptr(), inv_b.data_ptr(), _st())
+    return outs
+
+
+def _fp8_quant(xs, st, slot: int, e5m2: bool, row: bool = True, t: bool = True):
+    """Quantise the bf16 tensors `xs` with one dynamic scale, the amax over all of them, kept in row `slot` of the
+    device scale table st [n, 2] = (amax, 1/s).  Returns [(row-major, transposed)] per tensor."""
+    amax = st[slot, 0]
+    for x in xs:
+        fp8_amax(x, amax)
+    return [fp8_cast(x, amax, e5m2, row, t, inv=st[slot, 1]) for x in xs]
+
+
+def _fp8_dims(*dims):
+    """Every GEMM dimension of the FP8 block (and the row count) is a multiple of 16: 16-byte 8-bit TMA rows."""
+    bad = [int(v) for v in dims if int(v) % 16]
+    if bad:
+        raise _lib.TouchNetB200Error(f"float8_training: GEMM dimensions must be multiples of 16, got {bad}")
+
+
+# forward scale-table rows of the FP8 block: (amax, 1/s) of each GEMM input
+_F8_H1, _F8_WQKV, _F8_O, _F8_WO, _F8_H2, _F8_WGU, _F8_HM, _F8_WD = range(8)
+# backward rows: the incoming gradients
+_F8_D2, _F8_DG, _F8_DU, _F8_DX1, _F8_DQKV = range(5)
+
+
 def swiglu_bwd(g, u, dh, dg_out=None, du_out=None):
     M, N = g.shape
     dg = torch.empty_like(g) if dg_out is None else dg_out
@@ -674,13 +820,19 @@ def _unpad_heads(x: torch.Tensor, heads: int, hd: int) -> torch.Tensor:
 
 
 def block_forward(x2, ln1, wqb, wkb, wvb, bq, bk, bv, wob, ln2, wgb, wub, wdb, cos, sin, H, KV, eps, hd, attend, tp=None,
-                  need_gu=True, qkv_rows=None):
+                  need_gu=True, qkv_rows=None, fp8: bool = False):
     """Forward of one pre-norm decoder block on rows x2 [M, d] with bf16 working weights - the body shared by training
     (DecoderLayerFn), prompt prefill and cached decoding (generation.py), which differ only in `attend(q, k, v) ->
     (o, lse, k, v)`: q/k/v arrive projected, rotated and (head_dim < 128) zero-padded to 128-wide heads.
     `qkv_rows` (default M) is the row count the QKV path (fused with the RoPE epilogue, or not) is chosen for: a
     speculative verify step passes the decode step's B so that every row is computed as the decode step computes it.
-    Returns (out, saved) with saved = (rstd1, h1, q, k, v, o, lse, x1, rstd2, h2, g, u, hm) for the backward."""
+    Returns (out, saved) with saved = (rstd1, h1, q, k, v, o, lse, x1, rstd2, h2, g, u, hm) for the backward.
+    fp8=True (training only, no tensor parallelism): the seven projections run as FP8 GEMMs on dynamically scaled e4m3
+    copies of their inputs and weights; h1, h2 and hm in `saved` are then the transposed e4m3 copies the weight
+    gradients need, and saved ends with (oᵀ in e4m3, the scale table)."""
+    if fp8:
+        return _block_forward_fp8(x2, ln1, wqb, wkb, wvb, bq, bk, bv, wob, ln2, wgb, wub, wdb, cos, sin, H, KV, eps, hd,
+                                  attend)
     h1, _, rstd1 = rmsnorm_fwd(x2, ln1, eps)
     if tp is not None:
         h1 = tp.gather_rows(h1, keep=True)                               # [B*T, d]: every row, for the local heads
@@ -715,6 +867,114 @@ def block_forward(x2, ln1, wqb, wkb, wvb, bq, bk, bv, wob, ln2, wgb, wub, wdb, c
     return out, (rstd1, h1, q, k, v, o, lse, x1, rstd2, h2, g, u, hm)
 
 
+def _block_forward_fp8(x2, ln1, wqb, wkb, wvb, bq, bk, bv, wob, ln2, wgb, wub, wdb, cos, sin, H, KV, eps, hd, attend):
+    """block_forward with FP8 projections (see there).  q/k/v weights share one scale, as do gate/up: the fused QKV
+    dgrad sums over the three stacked weights and the SwiGLU tile holds gate and up rows, so one post-accumulation
+    scale must cover them."""
+    nq, nkv, d, ffn = wqb.shape[0], wkb.shape[0], wqb.shape[1], wgb.shape[0]
+    _fp8_dims(x2.shape[0], d, nq, nkv, wob.shape[1], ffn)
+    st = torch.zeros((8, 2), dtype=torch.float32, device=x2.device)
+    inv = st[:, 1]
+    h1, _, rstd1 = rmsnorm_fwd(x2, ln1, eps)
+    ((h1_8, h1_t),) = _fp8_quant([h1], st, _F8_H1, False)
+    wq8, wk8, wv8 = (w for w, _ in _fp8_quant([wqb, wkb, wvb], st, _F8_WQKV, False, t=False))
+    rope_in_gemm = qkv_fusable(h1.shape[0], nq, nkv) and bq is None and hd == 128
+    if qkv_fusable(h1.shape[0], nq, nkv):
+        qkv = gemm_qkv_fwd_fp8(h1_8, wq8, wk8, wv8, inv[_F8_H1], inv[_F8_WQKV], rope=(cos, sin) if rope_in_gemm else None)
+        q, k, v = qkv[:, :nq], qkv[:, nq:nq + nkv], qkv[:, nq + nkv:]
+    else:
+        q, k, v = (gemm_fp8(h1_8, w8, inv[_F8_H1], inv[_F8_WQKV]) for w8 in (wq8, wk8, wv8))
+    if bq is not None:
+        q += bq.to(BF16); k += bk.to(BF16); v += bv.to(BF16)
+    if not rope_in_gemm:
+        rope_apply_(q, cos, sin, H, hd)
+        rope_apply_(k, cos, sin, KV, hd)
+    if hd != 128:
+        q, k, v = _pad_heads(q, H, hd), _pad_heads(k, KV, hd), _pad_heads(v, KV, hd)
+    o, lse, k, v = attend(q, k, v)
+    ((o8, o_t),) = _fp8_quant([o if hd == 128 else _unpad_heads(o, H, hd)], st, _F8_O, False)
+    ((wo8, _),) = _fp8_quant([wob], st, _F8_WO, False, t=False)
+    x1 = gemm_fp8(o8, wo8, inv[_F8_O], inv[_F8_WO], residual=x2)
+    h2, _, rstd2 = rmsnorm_fwd(x1, ln2, eps)
+    ((h2_8, h2_t),) = _fp8_quant([h2], st, _F8_H2, False)
+    wg8, wu8 = (w for w, _ in _fp8_quant([wgb, wub], st, _F8_WGU, False, t=False))
+    g, u, hm = gemm_swiglu_fp8(h2_8, wg8, wu8, inv[_F8_H2], inv[_F8_WGU])
+    ((hm8, hm_t),) = _fp8_quant([hm], st, _F8_HM, False)
+    ((wd8, _),) = _fp8_quant([wdb], st, _F8_WD, False, t=False)
+    out = gemm_fp8(hm8, wd8, inv[_F8_HM], inv[_F8_WD], residual=x1)
+    return out, (rstd1, h1_t, q, k, v, o, lse, x1, rstd2, h2_t, g, u, hm_t, o_t, st)
+
+
+def _fp8_weight_t(wb, st, slot, out_t=None):
+    """The transposed e4m3 copy of bf16 weight wb [N, K] -> [K, N], at the scale the forward used (row `slot` of st)."""
+    return fp8_cast(wb, st[slot, 0], False, row=False, out_t=out_t)[1]
+
+
+def _block_backward_fp8(ctx, saved, d2):
+    """Weight and input gradients of the FP8 block: every incoming gradient is quantised to e5m2 (one scale for dq|dk|dv,
+    which the fused QKV dgrad sums over), dgrad = dY·Wᵀ and wgrad = dYᵀ·Xᵀ as FP8 GEMMs on K-major copies."""
+    (x2, ln1, ln2, wqb, wkb, wvb, wob, wgb, wub, wdb, cos, sin, rstd1, h1_t, q, k, v, o, lse, x1, rstd2, h2_t, g, u,
+     hm_t, o_t, st) = saved
+    H, KV, f32, hd = ctx.H, ctx.KV, ctx.f32, ctx.hd
+    M, dev = d2.shape[0], d2.device
+    inv = st[:, 1]
+    sb = torch.zeros((5, 2), dtype=torch.float32, device=dev)
+    ib = sb[:, 1]
+    # ---- MLP ----
+    ((d2_8, d2_t),) = _fp8_quant([d2], sb, _F8_D2, True)
+    dg, du = gemm_dswiglu_fp8(d2_8, _fp8_weight_t(wdb, st, _F8_WD), g, u, ib[_F8_D2], inv[_F8_WD])
+    dwd = gemm_fp8(d2_t, hm_t, ib[_F8_D2], inv[_F8_HM], out_f32=f32)
+    del d2_8, d2_t
+    ((dg8, dg_t),) = _fp8_quant([dg], sb, _F8_DG, True)
+    ((du8, du_t),) = _fp8_quant([du], sb, _F8_DU, True)
+    del dg, du
+    dh2 = gemm_fp8(dg8, _fp8_weight_t(wgb, st, _F8_WGU), ib[_F8_DG], inv[_F8_WGU])
+    dh2 = gemm_fp8(du8, _fp8_weight_t(wub, st, _F8_WGU), ib[_F8_DU], inv[_F8_WGU], residual=dh2, out=dh2)
+    dwg = gemm_fp8(dg_t, h2_t, ib[_F8_DG], inv[_F8_H2], out_f32=f32)
+    dwu = gemm_fp8(du_t, h2_t, ib[_F8_DU], inv[_F8_H2], out_f32=f32)
+    del dg8, dg_t, du8, du_t
+    dx1, dln2 = rmsnorm_bwd(x1, dh2, ln2, rstd2, ds_extra=d2)
+    # ---- attention ----
+    ((dx1_8, dx1_t),) = _fp8_quant([dx1], sb, _F8_DX1, True)
+    do = gemm_fp8(dx1_8, _fp8_weight_t(wob, st, _F8_WO), ib[_F8_DX1], inv[_F8_WO])
+    dwo = gemm_fp8(dx1_t, o_t, ib[_F8_DX1], inv[_F8_O], out_f32=f32)
+    del dx1_8, dx1_t
+    if hd != 128:   # padded heads: gradients of the padded tensors, un-padded, then the inverse rotation at head_dim hd
+        dq, dk, dv = attn_bwd(q, k, v, o, _pad_heads(do, H, hd), lse, ctx.plan, H, KV, ctx.scale)
+        dq, dk, dv = _unpad_heads(dq, H, hd), _unpad_heads(dk, KV, hd), _unpad_heads(dv, KV, hd)
+        rope_apply_(dq, cos, sin, H, hd, inverse=True)
+        rope_apply_(dk, cos, sin, KV, hd, inverse=True)
+    else:
+        dq, dk, dv = attn_bwd(q, k, v, o, do, lse, ctx.plan, H, KV, ctx.scale, rope=(cos, sin))
+    del do
+    nq, nkv = wqb.shape[0], wkb.shape[0]
+    tot, offs, widths = nq + 2 * nkv, (0, nq, nq + nkv), (nq, nkv, nkv)
+    dqkv8 = torch.empty((M, tot), dtype=F8E5M2, device=dev)
+    dqkv_t = torch.empty((tot, M), dtype=F8E5M2, device=dev)
+    for dy in (dq, dk, dv):
+        fp8_amax(dy, sb[_F8_DQKV, 0])
+    for dy, off, n in zip((dq, dk, dv), offs, widths):
+        fp8_cast(dy, sb[_F8_DQKV, 0], True, inv=ib[_F8_DQKV], out=dqkv8[:, off:off + n], out_t=dqkv_t[off:off + n])
+    w_t = torch.empty((wqb.shape[1], tot), dtype=F8E4M3, device=dev)   # [Wq;Wk;Wv]ᵀ
+    for wb, off, n in zip((wqb, wkb, wvb), offs, widths):
+        _fp8_weight_t(wb, st, _F8_WQKV, out_t=w_t[:, off:off + n])
+    if qkv_fusable(M, nq, nkv):
+        dh1 = gemm_qkv_dgrad_fp8(dqkv8, w_t, nq, nkv, ib[_F8_DQKV], inv[_F8_WQKV])
+        dwq, dwk, dwv = gemm_qkv_wgrad_fp8(dqkv_t, h1_t, f32, nq, nkv, ib[_F8_DQKV], inv[_F8_H1])
+    else:
+        dh1 = None
+        dws = []
+        for off, n in zip(offs, widths):
+            dh1 = gemm_fp8(dqkv8[:, off:off + n], w_t[:, off:off + n], ib[_F8_DQKV], inv[_F8_WQKV], residual=dh1, out=dh1)
+            dws.append(gemm_fp8(dqkv_t[off:off + n], h1_t, ib[_F8_DQKV], inv[_F8_H1], out_f32=f32))
+        dwq, dwk, dwv = dws
+    dbq = dbk = dbv = None
+    if ctx.has_bias:
+        dbq = dq.float().sum(0).to(ctx.w_dtype); dbk = dk.float().sum(0).to(ctx.w_dtype); dbv = dv.float().sum(0).to(ctx.w_dtype)
+    dx, dln1 = rmsnorm_bwd(x2, dh1, ln1, rstd1, ds_extra=dx1)
+    return dx, dln1.to(ln1.dtype), dwq, dwk, dwv, dbq, dbk, dbv, dwo, dln2.to(ln2.dtype), dwg, dwu, dwd
+
+
 class DecoderLayerFn(torch.autograd.Function):
     """One pre-norm decoder block as a single autograd node (hf: LlamaDecoderLayer.forward modeling_llama.py:303-333):
     7 kernel launches forward, residual adds fused into the o_proj / down_proj GEMM epilogues, q/k/v projections one
@@ -725,7 +985,7 @@ class DecoderLayerFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, ln1, wq, wk, wv, bq, bk, bv, wo, ln2, wg, wu, wd, wqb, wkb, wvb, wob, wgb, wub, wdb, cos, sin,
-                plan, H, KV, eps, hd=128):
+                plan, H, KV, eps, hd=128, fp8=False):
         x2 = _rows2d(x)
         scale = 1.0 / math.sqrt(hd)
         if hd != 128 and (hd > 128 or hd % 8 or plan.tp is not None or plan.cp_group is not None):
@@ -733,6 +993,8 @@ class DecoderLayerFn(torch.autograd.Function):
         tp = plan.tp                # tensor + sequence parallel: x holds T/tp rows, weights are this rank's shards
         if tp is not None and plan.cp_group is not None:
             raise _lib.TouchNetB200Error("tensor parallelism and context parallelism cannot be combined in one block")
+        if fp8 and (tp is not None or plan.cp_group is not None):
+            raise _lib.TouchNetB200Error("float8_training does not support tensor or context parallelism")
 
         def attend(q, k, v):
             if plan.cp_group is None:
@@ -743,24 +1005,25 @@ class DecoderLayerFn(torch.autograd.Function):
             return _cp.cp_attn_fwd(q, k, v, plan, H, KV, scale)
 
         out, saved = block_forward(x2, ln1, wqb, wkb, wvb, bq, bk, bv, wob, ln2, wgb, wub, wdb, cos, sin, H, KV, eps, hd,
-                                   attend, tp)
-        rstd1, h1, q, k, v, o, lse, x1, rstd2, h2, g, u, hm = saved
-        ctx.save_for_backward(x2, ln1, ln2, wqb, wkb, wvb, wob, wgb, wub, wdb, cos, sin, rstd1, h1, q, k, v, o, lse, x1,
-                              rstd2, h2, g, u, hm)
-        ctx.plan, ctx.H, ctx.KV, ctx.scale, ctx.has_bias, ctx.hd = plan, H, KV, scale, bq is not None, hd
+                                   attend, tp, fp8=fp8)
+        ctx.save_for_backward(x2, ln1, ln2, wqb, wkb, wvb, wob, wgb, wub, wdb, cos, sin, *saved)
+        ctx.plan, ctx.H, ctx.KV, ctx.scale, ctx.has_bias, ctx.hd, ctx.fp8 = plan, H, KV, scale, bq is not None, hd, fp8
         ctx.f32 = wq.dtype == torch.float32
         ctx.w_dtype = wq.dtype
         return out.view(x.shape)
 
     @staticmethod
     def backward(ctx, dout):
+        d2 = _rows2d(dout)
+        if d2.dtype != BF16:
+            d2 = d2.to(BF16)
+        if ctx.fp8:
+            dx, *grads = _block_backward_fp8(ctx, ctx.saved_tensors, d2)
+            return (dx.view(dout.shape), *grads) + (None,) * 15
         (x2, ln1, ln2, wqb, wkb, wvb, wob, wgb, wub, wdb, cos, sin, rstd1, h1, q, k, v, o, lse, x1, rstd2, h2, g, u,
          hm) = ctx.saved_tensors
         H, KV, f32 = ctx.H, ctx.KV, ctx.f32
         tp = ctx.plan.tp
-        d2 = _rows2d(dout)
-        if d2.dtype != BF16:
-            d2 = d2.to(BF16)
         # ---- MLP ----
         d2f = d2 if tp is None else tp.gather_rows(d2)     # backward of the forward reduce-scatter
         dg, du = gemm_dswiglu(d2f, wdb, g, u)          # down-proj dgrad, SwiGLU backward in its epilogue
@@ -824,10 +1087,11 @@ class DecoderLayerFn(torch.autograd.Function):
             tp.all_reduce_(dln1)
             tp.all_reduce_(dln2)
         return (dx.view(dout.shape), dln1.to(ln1.dtype), dwq, dwk, dwv, dbq, dbk, dbv, dwo, dln2.to(ln2.dtype), dwg, dwu,
-                dwd) + (None,) * 14
+                dwd) + (None,) * 15
 
 
-def decoder_layer(x, ln1, wq, wk, wv, bq, bk, bv, wo, ln2, wg, wu, wd, cos, sin, plan, H, KV, eps, hd=128):
+def decoder_layer(x, ln1, wq, wk, wv, bq, bk, bv, wo, ln2, wg, wu, wd, cos, sin, plan, H, KV, eps, hd=128, fp8=False):
+    """`fp8`: the seven projections in FP8 (the `float8_training` model config key; see block_forward)."""
     return DecoderLayerFn.apply(x, ln1, wq, wk, wv, bq, bk, bv, wo, ln2, wg, wu, wd, bf16_weight(wq), bf16_weight(wk),
                                 bf16_weight(wv), bf16_weight(wo), bf16_weight(wg), bf16_weight(wu), bf16_weight(wd),
-                                cos, sin, plan, H, KV, eps, hd)
+                                cos, sin, plan, H, KV, eps, hd, fp8)
