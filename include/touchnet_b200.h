@@ -111,6 +111,38 @@ int tn_fp8_amax_bf16(const void* x, int64_t ldx, int64_t rows, int64_t cols, flo
 int tn_fp8_cast_bf16(const void* x, int64_t ldx, int64_t rows, int64_t cols, int e5m2, const float* amax, void* out,
                      int64_t ld_out, void* out_t, int64_t ld_out_t, float* inv_scale, tn_stream_t stream);
 
+/* Rowwise FP8 (torchao's rowwise recipe, opt-in through the model config key `float8_recipe_name`): e4m3 operands with
+ * one power-of-two scale per row along the GEMM's reduction axis, s = 2^floor(log2(448 / max(amax, 1e-12))) with the
+ * division in fp64 and the result in fp32.  bf16 [rows, cols] views, rows and cols multiples of 16; NaN stays NaN.
+ *   tn_fp8_rowwise_cast_bf16  : out = sat_rne(x · s_row) row-major [rows, cols], inv_scale[rows] = 1/s_row.
+ *   tn_fp8_colwise_amax_bf16  : amax[c] = max(amax[c], max_r |x[r,c]|) (atomic; the caller zeroes amax[cols]; several
+ *                               calls share one vector).
+ *   tn_fp8_colwise_cast_t_bf16: out_t = sat_rne(x · s_col)ᵀ [cols, rows] with s_col from amax[cols]; inv_scale[cols] =
+ *                               1/s_col if inv_scale is not NULL.
+ * GEMMs: as the tensorwise twins with A and B e4m3 and 1/s vectors over the rows of A (inv_sa [M]) and of B (inv_sb
+ * [N]; SwiGLU: inv_sw [2N], the gate rows then the up rows; QKV mode 0: over the rows of [Wq;Wk;Wv]).  Each accumulator
+ * element is multiplied with the 1/s of its row and column.  tn_gemm_fp8_rowwise accumulates in the tensor-core
+ * accumulator, or with `promoted` in a separate fp32 accumulator per 128-k stage; dSwiGLU and QKV modes 1 and 2 always
+ * promote, SwiGLU and QKV mode 0 never do.  Scale vectors are 8 B aligned. */
+int tn_fp8_rowwise_cast_bf16(const void* x, int64_t ldx, int64_t rows, int64_t cols, void* out, int64_t ld_out,
+                             float* inv_scale, tn_stream_t stream);
+int tn_fp8_colwise_amax_bf16(const void* x, int64_t ldx, int64_t rows, int64_t cols, float* amax, tn_stream_t stream);
+int tn_fp8_colwise_cast_t_bf16(const void* x, int64_t ldx, int64_t rows, int64_t cols, const float* amax, void* out_t,
+                               int64_t ld_out_t, float* inv_scale, tn_stream_t stream);
+int tn_gemm_fp8_rowwise(const void* A, int64_t lda, const void* B, int64_t ldb, void* D, int64_t ldd, int d_f32,
+                        const void* R, int64_t ldr, int M, int N, int K, const float* inv_sa, const float* inv_sb,
+                        int promoted, tn_stream_t stream);
+int tn_gemm_swiglu_fp8_rowwise(const void* X, int64_t ldx, const void* Wg, const void* Wu, int64_t ldw, void* G,
+                               void* U, void* H, int64_t ldh, int M, int N, int K, const float* inv_sx,
+                               const float* inv_sw, tn_stream_t stream);
+int tn_gemm_dswiglu_fp8_rowwise(const void* dY, int64_t lddy, const void* W, int64_t ldw, const void* G, const void* U,
+                                int64_t ldgu, void* dG, void* dU, int64_t lddg, int M, int N, int K,
+                                const float* inv_sa, const float* inv_sb, tn_stream_t stream);
+int tn_gemm_qkv_fp8_rowwise(int mode, const void* A, int64_t lda, const void* B0, const void* B1, const void* B2,
+                            int64_t ldb, void* D0, void* D1, void* D2, int64_t ldd, int d_f32, int s0, int s1, int s2,
+                            int M, int N, int K, const void* rope_cos, const void* rope_sin, const float* inv_sa,
+                            const float* inv_sb, tn_stream_t stream);
+
 /* SwiGLU backward (elementwise): dG = dH⊙U⊙silu'(G), dU = dH⊙silu(G).  bf16 [M,N] contiguous rows (ld). */
 int tn_swiglu_bwd_bf16(const void* G, const void* U, const void* dH, void* dG, void* dU, int64_t rows, int64_t cols,
                        int64_t ld, tn_stream_t stream);

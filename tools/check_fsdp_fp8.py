@@ -1,10 +1,11 @@
 """FP8 training (config key `float8_training`) under FSDP2 against the same FP8 model on one GPU without FSDP.
-    torchrun --nproc-per-node N tools/check_fsdp_fp8.py        (N = 1 runs FSDP2 on a one-rank mesh)
+    torchrun --nproc-per-node N tools/check_fsdp_fp8.py [--recipe tensorwise|rowwise]   (N = 1: a one-rank mesh)
 Each rank trains on its own packed row.  The single-GPU reference runs that row with fp32 master weights (the block casts
 them to bf16 itself); under FSDP2 the block receives the bf16 all-gathered parameters.  Both hand the FP8 block the same
 bf16 weights and the same row, so each rank's loss must be bitwise equal.  The reduced gradients are compared with the
 sum of the reference gradients over the ranks: FSDP2 computes bf16 weight gradients and reduces them in fp32, the
 reference computes fp32 ones, so they agree to bf16 rounding."""
+import argparse
 import os
 import sys
 
@@ -18,6 +19,9 @@ from tests.gpu_util import packed_doc_ids, rel_err  # noqa: E402
 from tests.test_gpu_model import small_cfg  # noqa: E402
 from touchnet_b200 import modeling  # noqa: E402
 
+ap = argparse.ArgumentParser()
+ap.add_argument("--recipe", default="tensorwise", help="float8_recipe_name: tensorwise or rowwise")
+args = ap.parse_args()
 rank, world = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"])
 dev = torch.device("cuda", int(os.environ.get("LOCAL_RANK", rank)))
 torch.cuda.set_device(dev)
@@ -33,6 +37,7 @@ with torch.no_grad():
 for p in model.parameters():
     dist.broadcast(p.data, 0)
 model.float8_training = True
+model.float8_recipe_name = args.recipe
 T = 1024
 lens = [[300, 500, 100], [1024], [512, 512], [1000]][:world]
 doc, pos = packed_doc_ids(world, T, lens, dev)
@@ -78,7 +83,7 @@ for n, p in model.named_parameters():
 flags = torch.tensor([0 if same else 1], device=dev)
 dist.all_reduce(flags)
 if rank == 0:
-    print(f"FSDP{world} FP8: loss {loss.item():.6f} vs {ref_loss.item():.6f} (bitwise on every rank: {int(flags) == 0}); "
+    print(f"FSDP{world} FP8 ({args.recipe}): loss {loss.item():.6f} vs {ref_loss.item():.6f} (bitwise on every rank: {int(flags) == 0}); "
           f"worst grad rel err {worst:.4g}")
     assert int(flags) == 0 and worst < 1e-2
     print("FSDP FP8 OK")

@@ -23,6 +23,10 @@
 // (e4m3 A) accumulates in the wgmma accumulator alone; dgrad and wgrad (e5m2 A) add each stage's partial sum into a
 // separate fp32 accumulator, because the 8-bit MMAs accumulate with reduced precision.  That doubles the accumulator
 // registers, so the promoted form runs on the 128-wide tile only.
+// Rowwise FP8 (OP 3, 4): both operands e4m3 with one scale per row of A and per row of B (torchao's rowwise recipe,
+// torch._scaled_mm's scale_a [M,1] / scale_b [1,N]); the dequantisation multiplies each accumulator element with the
+// 1/s of its row and its column, read from two device vectors, ahead of the same epilogues.  OP 3 accumulates like
+// OP 1 (forward), OP 4 promotes like OP 2 (dgrad, wgrad).
 #include <stdio.h>
 #include <stdlib.h>
 
@@ -75,6 +79,8 @@ struct GemmParams {
   const bf16* aux_u;
   int64_t ld_gu;
   // FP8: 1/s of the A and B operands (device floats written by tn_fp8_cast_bf16)
+  // rowwise FP8: vectors of 1/s per row of A [M] and per row of B [N] (the QKV forward: the rows of [Wq;Wk;Wv],
+  // indexed by the output column; EPI 1: [2N], the gate rows then the up rows)
   const float* inv_sa;
   const float* inv_sb;
 };
@@ -96,12 +102,13 @@ __device__ __forceinline__ void decode_tile(int tile, int num_m, int num_n, int 
 }
 
 // OP: operand type and accumulation.  0 = bf16;  1 = e4m3 A, e4m3 B, accumulated in the wgmma accumulator (forward);
-//     2 = e5m2 A, e4m3 B, stage partial sums promoted into a separate fp32 accumulator (dgrad / wgrad, BN 128 only)
+//     2 = e5m2 A, e4m3 B, stage partial sums promoted into a separate fp32 accumulator (dgrad / wgrad, BN 128 only);
+//     3 = OP 1 and 4 = e4m3 A promoted as OP 2, both with per-row scales (rowwise recipe)
 template <int BN, bool A_MN, bool B_MN, int EPI, int OP = 0>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_kernel(const __grid_constant__ GemmMaps tm, const GemmParams p) {
   static_assert(OP == 0 || (!A_MN && !B_MN), "8-bit operands are K-major");
-  static_assert(OP != 2 || BN == 128, "the promoted accumulator fits the 128-wide tile only");
+  static_assert((OP != 2 && OP != 4) || BN == 128, "the promoted accumulator fits the 128-wide tile only");
   using C = TileCfg<BN>;
   constexpr int STAGES = C::STAGES;
   extern __shared__ uint8_t smem_raw[];
@@ -259,11 +266,11 @@ gemm_kernel(const __grid_constant__ GemmMaps tm, const GemmParams p) {
       const uint32_t a_addr = smem_u32(sA + stage * A_BYTES) + uint32_t(c) * 8192u;
       const uint32_t b_addr = smem_u32(sB + stage * C::B_BYTES);
       wgmma_fence();
-      if constexpr (OP == 2) {
+      if constexpr (OP == 2 || OP == 4) {
         float part[BN / 2];                      // this stage's partial sum
 #pragma unroll
         for (int k = 0; k < 4; ++k)
-          wgmma_fp8_m64n128<true>(part, make_sdesc_sw128(a_addr + k * 32, 16, 1024),
+          wgmma_fp8_m64n128<OP == 2>(part, make_sdesc_sw128(a_addr + k * 32, 16, 1024),
                                   make_sdesc_sw128(b_addr + k * 32, 16, 1024), k > 0 ? 1u : 0u);
         wgmma_commit();
         wgmma_wait<0>();
@@ -275,7 +282,7 @@ gemm_kernel(const __grid_constant__ GemmMaps tm, const GemmParams p) {
         for (int k = 0; k < BK / 16; ++k) {
           const uint64_t da = A_MN ? make_sdesc_sw128(a_addr + k * 2048, 8192, 1024) : make_sdesc_sw128(a_addr + k * 32, 16, 1024);
           const uint64_t db = B_MN ? make_sdesc_sw128(b_addr + k * 2048, 8192, 1024) : make_sdesc_sw128(b_addr + k * 32, 16, 1024);
-          if constexpr (OP == 1) {
+          if constexpr (OP == 1 || OP == 3) {
             if constexpr (BN == 256) wgmma_fp8_m64n256<false>(acc, da, db, 1u);
             else wgmma_fp8_m64n128<false>(acc, da, db, 1u);
           } else if constexpr (BN == 256) {
@@ -295,10 +302,37 @@ gemm_kernel(const __grid_constant__ GemmMaps tm, const GemmParams p) {
     wgmma_wait<0>();
     wgmma_fence_regs(acc);
     if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
-    if constexpr (OP != 0) {   // dequantise: acc · (1/s_a)·(1/s_b), ahead of every epilogue
+    if constexpr (OP == 1 || OP == 2) {   // dequantise: acc · (1/s_a)·(1/s_b), ahead of every epilogue
       const float sc = *p.inv_sa * *p.inv_sb;
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) acc[i] *= sc;
+    } else if constexpr (OP >= 3) {       // acc(m, n) · (1/s_a[m]) · (1/s_b[n]); rows / columns past M / N are clipped
+      const int row = m_blk * BM + c * 64 + r_loc;
+      float sa[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) sa[h] = row + 8 * h < p.M ? p.inv_sa[row + 8 * h] : 0.f;
+      // the 1/s of columns 8j + cq, +1: lane L loads those of j = 8g + L/4 for the threads with lane % 4 == L % 4 and
+      // hands them out by shuffle (one coalesced load per 8 j; per-j loads would be hoisted next to the live
+      // accumulator and spill on the 256-wide tile)
+#pragma unroll
+      for (int g = 0; g < BN / 64; ++g) {
+        const int jl = 8 * g + (lane >> 2);
+        const bool up = EPI == 1 && jl >= BN / 16;       // SwiGLU: the up half of the tile
+        const int col = n_blk * TN + 8 * (up ? jl - BN / 16 : jl) + cq;
+        const float2 sb = col < p.N ? *reinterpret_cast<const float2*>(p.inv_sb + (up ? p.N : 0) + col)
+                                    : make_float2(0.f, 0.f);
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+          const int j = 8 * g + jj, src = (jj << 2) | (lane & 3);
+          const float bx = __shfl_sync(0xffffffffu, sb.x, src), by = __shfl_sync(0xffffffffu, sb.y, src);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            acc[4 * j + 2 * h] = acc[4 * j + 2 * h] * sa[h] * bx;
+            acc[4 * j + 2 * h + 1] = acc[4 * j + 2 * h + 1] * sa[h] * by;
+          }
+        }
+      }
+      wgmma_fence_regs(acc);   // keeps the products here: sunk into the epilogue, the 64 scales would stay live there
     }
 
     // ---------------- epilogue: registers -> swizzled staging (-> coalesced pass) -> TMA store ----------------
@@ -552,14 +586,31 @@ static int map_operand_fp8(CUtensorMap* m, const void* ptr, uint64_t rows, uint6
   return encode_tmap_2d(m, ptr, 1, K, rows, uint64_t(ld), 128, box_rows, true);
 }
 
-// FP8 launches: the operand type of A selects the accumulation (see gemm_kernel's OP), the promoted form the 128 tile
-static int fp8_bn(int a_e5m2, int M, int N, int out_div) { return a_e5m2 ? 128 : pick_bn(M, N, out_div); }
-
+// FP8 launches: `op` is gemm_kernel's OP (1-4).  The promoted forms (2, 4) run on the 128 tile, and so do the rowwise
+// SwiGLU and fp32-output forms (EPI 1, 2), which spill on the 256 tile: the per-column scales cost registers there.
 template <int EPI>
-static int launch_fp8(int a_e5m2, int bn, const GemmMaps& tm, const GemmParams& p, cudaStream_t stream) {
-  if (a_e5m2) return launch_gemm<128, false, false, EPI, 2>(tm, p, stream);
-  return bn == 256 ? launch_gemm<256, false, false, EPI, 1>(tm, p, stream)
-                   : launch_gemm<128, false, false, EPI, 1>(tm, p, stream);
+static bool fp8_wide_ok(int op) { return op == 1 || (op == 3 && EPI != 1 && EPI != 2); }
+template <int EPI>
+static int fp8_bn(int op, int M, int N, int out_div) { return fp8_wide_ok<EPI>(op) ? pick_bn(M, N, out_div) : 128; }
+
+// Rowwise forms exist where an entry point can reach them: the SwiGLU forward (EPI 1) never promotes, the dSwiGLU
+// backward (EPI 3) always does.
+template <int EPI>
+static int launch_fp8(int op, int bn, const GemmMaps& tm, const GemmParams& p, cudaStream_t stream) {
+  if (op == 1)
+    return bn == 256 ? launch_gemm<256, false, false, EPI, 1>(tm, p, stream)
+                     : launch_gemm<128, false, false, EPI, 1>(tm, p, stream);
+  if (op == 2) return launch_gemm<128, false, false, EPI, 2>(tm, p, stream);
+  if constexpr (EPI != 3) {
+    if (op == 3) {
+      if constexpr (EPI != 1 && EPI != 2)
+        if (bn == 256) return launch_gemm<256, false, false, EPI, 3>(tm, p, stream);
+      return launch_gemm<128, false, false, EPI, 3>(tm, p, stream);
+    }
+  }
+  if constexpr (EPI != 1)
+    if (op == 4) return launch_gemm<128, false, false, EPI, 4>(tm, p, stream);
+  return fail(TN_ERR_UNSUPPORTED, "FP8 GEMM: operand mode %d is not built for epilogue %d", op, EPI);
 }
 
 static GemmParams fp8_params(int M, int N, int K, int tile_n, const float* inv_sa, const float* inv_sb) {
@@ -726,27 +777,31 @@ extern "C" int tn_gemm_qkv_bf16(int mode, const void* A, int64_t lda, const void
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// FP8 twins of the entry points above: K-major 8-bit operands (A e4m3, or e5m2 with a_e5m2; B e4m3), 1/s_a and 1/s_b
-// read from device memory (tn_fp8_cast_bf16), outputs and epilogues as in the bf16 entry points.  Every dimension and
-// leading dimension is a multiple of 16 (TMA rows of 8-bit elements are 16-byte aligned).
+// FP8 twins of the entry points above: K-major 8-bit operands, outputs and epilogues as in the bf16 entry points.
+// Tensorwise (tn_*_fp8): A e4m3, or e5m2 with a_e5m2 (promoted accumulation); B e4m3; 1/s_a and 1/s_b are single
+// device floats (tn_fp8_cast_bf16).  Rowwise (tn_*_fp8_rowwise): A and B e4m3, 1/s_a and 1/s_b are device vectors
+// over the rows of A and of B (tn_fp8_rowwise_cast_bf16, tn_fp8_colwise_cast_t_bf16).  Every dimension and leading
+// dimension is a multiple of 16 (TMA rows of 8-bit elements are 16-byte aligned).
 // ---------------------------------------------------------------------------------------------------------------
 #define TN_FP8_REQUIRE_COMMON(name, A, lda, B, ldb, inv_sa, inv_sb, M, N, K)                                          \
-  TN_REQUIRE(A && B && inv_sa && inv_sb, name ": null pointer");                                                    \
+  TN_REQUIRE(A && B && inv_sa && inv_sb, "%s: null pointer", name);                                                 \
   TN_REQUIRE(M > 0 && N > 0 && K > 0 && M % 16 == 0 && N % 16 == 0 && K % 16 == 0,                                   \
-             name ": M=%d N=%d K=%d must be positive multiples of 16", M, N, K);                                      \
+             "%s: M=%d N=%d K=%d must be positive multiples of 16", name, M, N, K);                                   \
   TN_REQUIRE(lda % 16 == 0 && ldb % 16 == 0 && aligned16(A) && aligned16(B),                                        \
-             name ": A and B must be 16 B aligned with leading dims that are multiples of 16")
+             "%s: A and B must be 16 B aligned with leading dims that are multiples of 16", name)
+// rowwise scale vectors are read in pairs
+#define TN_FP8_REQUIRE_VEC(name, v) \
+  TN_REQUIRE((reinterpret_cast<uintptr_t>(v) & 7) == 0, "%s: scale vectors must be 8 B aligned", name)
 
-extern "C" int tn_gemm_fp8(const void* A, int64_t lda, int a_e5m2, const void* B, int64_t ldb, void* D, int64_t ldd,
-                           int d_f32, const void* R, int64_t ldr, int M, int N, int K, const float* inv_sa,
-                           const float* inv_sb, tn_stream_t stream_) {
-  clear_error();
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  TN_REQUIRE(D, "tn_gemm_fp8: null pointer");
-  TN_FP8_REQUIRE_COMMON("tn_gemm_fp8", A, lda, B, ldb, inv_sa, inv_sb, M, N, K);
-  TN_REQUIRE(ldd % (d_f32 ? 4 : 8) == 0 && (!R || ldr % (d_f32 ? 4 : 8) == 0), "tn_gemm_fp8: ldd/ldr alignment");
-  TN_REQUIRE(aligned16(D) && (!R || aligned16(R)), "tn_gemm_fp8: D/R must be 16 B aligned");
-  const int bn = fp8_bn(a_e5m2, M, N, 1);
+static int gemm_fp8(const char* name, int op, const void* A, int64_t lda, const void* B, int64_t ldb, void* D,
+                    int64_t ldd, int d_f32, const void* R, int64_t ldr, int M, int N, int K, const float* inv_sa,
+                    const float* inv_sb, cudaStream_t stream) {
+  TN_REQUIRE(D, "%s: null pointer", name);
+  TN_FP8_REQUIRE_COMMON(name, A, lda, B, ldb, inv_sa, inv_sb, M, N, K);
+  TN_REQUIRE(ldd % (d_f32 ? 4 : 8) == 0 && (!R || ldr % (d_f32 ? 4 : 8) == 0), "%s: ldd/ldr alignment", name);
+  TN_REQUIRE(aligned16(D) && (!R || aligned16(R)), "%s: D/R must be 16 B aligned", name);
+  if (op >= 3) { TN_FP8_REQUIRE_VEC(name, inv_sa); TN_FP8_REQUIRE_VEC(name, inv_sb); }
+  const int bn = d_f32 ? fp8_bn<2>(op, M, N, 1) : fp8_bn<0>(op, M, N, 1);
   GemmParams p = fp8_params(M, N, K, bn, inv_sa, inv_sb);
   p.R = R; p.ldr = ldr;
   GemmMaps tm;
@@ -756,19 +811,18 @@ extern "C" int tn_gemm_fp8(const void* A, int64_t lda, int a_e5m2, const void* B
   if ((rc = map_output(&tm.d[0], D, d_f32, uint64_t(M), uint64_t(N), ldd))) return rc;
   tm.b[1] = tm.b[2] = tm.b[0];
   tm.d[1] = tm.d[2] = tm.d[0];
-  return d_f32 ? launch_fp8<2>(a_e5m2, bn, tm, p, stream) : launch_fp8<0>(a_e5m2, bn, tm, p, stream);
+  return d_f32 ? launch_fp8<2>(op, bn, tm, p, stream) : launch_fp8<0>(op, bn, tm, p, stream);
 }
 
-extern "C" int tn_gemm_swiglu_fp8(const void* X, int64_t ldx, int x_e5m2, const void* Wg, const void* Wu, int64_t ldw,
-                                  void* G, void* U, void* H, int64_t ldh, int M, int N, int K, const float* inv_sx,
-                                  const float* inv_sw, tn_stream_t stream_) {
-  clear_error();
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  TN_REQUIRE(Wu && H, "tn_gemm_swiglu_fp8: null pointer");
-  TN_FP8_REQUIRE_COMMON("tn_gemm_swiglu_fp8", X, ldx, Wg, ldw, inv_sx, inv_sw, M, N, K);
-  TN_REQUIRE(ldh % 8 == 0 && aligned16(Wu), "tn_gemm_swiglu_fp8: ldh must be a multiple of 8, Wu 16 B aligned");
-  TN_REQUIRE(aligned16(H) && (!G || aligned16(G)) && (!U || aligned16(U)), "tn_gemm_swiglu_fp8: outputs must be 16 B aligned");
-  const int bn = fp8_bn(x_e5m2, M, N, 2);
+static int gemm_swiglu_fp8(const char* name, int op, const void* X, int64_t ldx, const void* Wg, const void* Wu,
+                           int64_t ldw, void* G, void* U, void* H, int64_t ldh, int M, int N, int K, const float* inv_sx,
+                           const float* inv_sw, cudaStream_t stream) {
+  TN_REQUIRE(Wu && H, "%s: null pointer", name);
+  TN_FP8_REQUIRE_COMMON(name, X, ldx, Wg, ldw, inv_sx, inv_sw, M, N, K);
+  TN_REQUIRE(ldh % 8 == 0 && aligned16(Wu), "%s: ldh must be a multiple of 8, Wu 16 B aligned", name);
+  TN_REQUIRE(aligned16(H) && (!G || aligned16(G)) && (!U || aligned16(U)), "%s: outputs must be 16 B aligned", name);
+  if (op >= 3) { TN_FP8_REQUIRE_VEC(name, inv_sx); TN_FP8_REQUIRE_VEC(name, inv_sw); }
+  const int bn = fp8_bn<1>(op, M, N, 2);
   GemmParams p = fp8_params(M, N, K, bn / 2, inv_sx, inv_sw);
   p.has_g = G != nullptr; p.has_u = U != nullptr;
   GemmMaps tm;
@@ -781,22 +835,20 @@ extern "C" int tn_gemm_swiglu_fp8(const void* X, int64_t ldx, int x_e5m2, const 
   tm.d[1] = tm.d[2] = tm.d[0];
   if (G && (rc = map_output(&tm.d[1], G, 0, uint64_t(M), uint64_t(N), ldh))) return rc;
   if (U && (rc = map_output(&tm.d[2], U, 0, uint64_t(M), uint64_t(N), ldh))) return rc;
-  return launch_fp8<1>(x_e5m2, bn, tm, p, stream);
+  return launch_fp8<1>(op, bn, tm, p, stream);
 }
 
-// W is the K-major transposed copy of down_proj.weight: [N = ffn, K = d]
-extern "C" int tn_gemm_dswiglu_fp8(const void* dY, int64_t lddy, int dy_e5m2, const void* W, int64_t ldw, const void* G,
-                                   const void* U, int64_t ldgu, void* dG, void* dU, int64_t lddg, int M, int N, int K,
-                                   const float* inv_sa, const float* inv_sb, tn_stream_t stream_) {
-  clear_error();
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  TN_REQUIRE(G && U && dG && dU, "tn_gemm_dswiglu_fp8: null pointer");
-  TN_FP8_REQUIRE_COMMON("tn_gemm_dswiglu_fp8", dY, lddy, W, ldw, inv_sa, inv_sb, M, N, K);
-  TN_REQUIRE(M >= 256 && N >= 256, "tn_gemm_dswiglu_fp8: needs M, N >= 256");
-  TN_REQUIRE(ldgu % 8 == 0 && lddg % 8 == 0, "tn_gemm_dswiglu_fp8: ldgu and lddg must be multiples of 8");
-  TN_REQUIRE(aligned16(G) && aligned16(U) && aligned16(dG) && aligned16(dU),
-             "tn_gemm_dswiglu_fp8: G, U, dG, dU must be 16 B aligned");
-  const int bn = fp8_bn(dy_e5m2, M, N, 1);
+static int gemm_dswiglu_fp8(const char* name, int op, const void* dY, int64_t lddy, const void* W, int64_t ldw,
+                            const void* G, const void* U, int64_t ldgu, void* dG, void* dU, int64_t lddg, int M, int N,
+                            int K, const float* inv_sa, const float* inv_sb, cudaStream_t stream) {
+  TN_REQUIRE(G && U && dG && dU, "%s: null pointer", name);
+  TN_FP8_REQUIRE_COMMON(name, dY, lddy, W, ldw, inv_sa, inv_sb, M, N, K);
+  TN_REQUIRE(M >= 256 && N >= 256, "%s: needs M, N >= 256", name);
+  TN_REQUIRE(ldgu % 8 == 0 && lddg % 8 == 0, "%s: ldgu and lddg must be multiples of 8", name);
+  TN_REQUIRE(aligned16(G) && aligned16(U) && aligned16(dG) && aligned16(dU), "%s: G, U, dG, dU must be 16 B aligned",
+             name);
+  if (op >= 3) { TN_FP8_REQUIRE_VEC(name, inv_sa); TN_FP8_REQUIRE_VEC(name, inv_sb); }
+  const int bn = fp8_bn<3>(op, M, N, 1);
   GemmParams p = fp8_params(M, N, K, bn, inv_sa, inv_sb);
   p.aux_g = static_cast<const bf16*>(G); p.aux_u = static_cast<const bf16*>(U); p.ld_gu = ldgu;
   GemmMaps tm;
@@ -807,34 +859,33 @@ extern "C" int tn_gemm_dswiglu_fp8(const void* dY, int64_t lddy, int dy_e5m2, co
   if ((rc = map_output(&tm.d[0], dG, 0, uint64_t(M), uint64_t(N), lddg))) return rc;
   if ((rc = map_output(&tm.d[1], dU, 0, uint64_t(M), uint64_t(N), lddg))) return rc;
   tm.d[2] = tm.d[1];
-  return launch_fp8<3>(dy_e5m2, bn, tm, p, stream);
+  return launch_fp8<3>(op, bn, tm, p, stream);
 }
 
-// Modes as tn_gemm_qkv_bf16, all operands K-major: 1 = dgrad with B_i the [N, s_i] column blocks of Wᵀ (row stride
-// ldb), 2 = wgrad with A = the transposed gradient [s0+s1+s2, K] and B0 = the transposed layer input [N, K].
-extern "C" int tn_gemm_qkv_fp8(int mode, const void* A, int64_t lda, int a_e5m2, const void* B0, const void* B1,
-                               const void* B2, int64_t ldb, void* D0, void* D1, void* D2, int64_t ldd, int d_f32, int s0,
-                               int s1, int s2, int M, int N, int K, const void* rope_cos, const void* rope_sin,
-                               const float* inv_sa, const float* inv_sb, tn_stream_t stream_) {
-  clear_error();
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  TN_REQUIRE(D0, "tn_gemm_qkv_fp8: null pointer");
-  TN_FP8_REQUIRE_COMMON("tn_gemm_qkv_fp8", A, lda, B0, ldb, inv_sa, inv_sb, M, N, K);
-  TN_REQUIRE(mode >= 0 && mode <= 2, "tn_gemm_qkv_fp8: mode must be 0 (forward), 1 (dgrad) or 2 (wgrad)");
+// `op_fwd` is the OP of mode 0, `op_bwd` that of modes 1 and 2
+static int gemm_qkv_fp8(const char* name, int op_fwd, int op_bwd, int mode, const void* A, int64_t lda,
+                        const void* B0, const void* B1, const void* B2, int64_t ldb, void* D0, void* D1, void* D2,
+                        int64_t ldd, int d_f32, int s0, int s1, int s2, int M, int N, int K, const void* rope_cos,
+                        const void* rope_sin, const float* inv_sa, const float* inv_sb, cudaStream_t stream) {
+  TN_REQUIRE(D0, "%s: null pointer", name);
+  TN_FP8_REQUIRE_COMMON(name, A, lda, B0, ldb, inv_sa, inv_sb, M, N, K);
+  TN_REQUIRE(mode >= 0 && mode <= 2, "%s: mode must be 0 (forward), 1 (dgrad) or 2 (wgrad)", name);
   TN_REQUIRE(s0 > 0 && s1 > 0 && s2 > 0 && s0 % 256 == 0 && s1 % 256 == 0 && s2 % 256 == 0,
-             "tn_gemm_qkv_fp8: segment sizes (%d,%d,%d) must be positive multiples of 256", s0, s1, s2);
+             "%s: segment sizes (%d,%d,%d) must be positive multiples of 256", name, s0, s1, s2);
   const int tot = s0 + s1 + s2;
   TN_REQUIRE((mode == 0 && N == tot) || (mode == 1 && K == tot) || (mode == 2 && M == tot),
-             "tn_gemm_qkv_fp8: segments do not add up to the segmented dimension");
+             "%s: segments do not add up to the segmented dimension", name);
   TN_REQUIRE(M >= 256 && N >= 256 && ldd % (d_f32 ? 4 : 8) == 0,
-             "tn_gemm_qkv_fp8: needs M,N >= 256 and 16-byte aligned leading dimensions");
-  TN_REQUIRE(mode == 2 || (B1 && B2 && aligned16(B1) && aligned16(B2)), "tn_gemm_qkv_fp8: B1/B2 required, 16 B aligned");
-  TN_REQUIRE(mode != 2 || (D1 && D2), "tn_gemm_qkv_fp8: D1/D2 required for wgrad");
-  TN_REQUIRE((rope_cos == nullptr) == (rope_sin == nullptr), "tn_gemm_qkv_fp8: cos and sin tables come in pairs");
-  TN_REQUIRE(rope_cos == nullptr || mode == 0, "tn_gemm_qkv_fp8: fused RoPE exists for the forward projection only");
+             "%s: needs M,N >= 256 and 16-byte aligned leading dimensions", name);
+  TN_REQUIRE(mode == 2 || (B1 && B2 && aligned16(B1) && aligned16(B2)), "%s: B1/B2 required, 16 B aligned", name);
+  TN_REQUIRE(mode != 2 || (D1 && D2), "%s: D1/D2 required for wgrad", name);
+  TN_REQUIRE((rope_cos == nullptr) == (rope_sin == nullptr), "%s: cos and sin tables come in pairs", name);
+  TN_REQUIRE(rope_cos == nullptr || mode == 0, "%s: fused RoPE exists for the forward projection only", name);
+  const int op = mode == 0 ? op_fwd : op_bwd;
+  if (op >= 3) { TN_FP8_REQUIRE_VEC(name, inv_sa); TN_FP8_REQUIRE_VEC(name, inv_sb); }
   const void* Bs[3] = {B0, B1, B2};
   const int seg[3] = {s0, s1, s2};
-  const int bn = fp8_bn(a_e5m2, M, N, 1);
+  const int bn = mode == 2 && d_f32 ? fp8_bn<2>(op, M, N, 1) : fp8_bn<0>(op, M, N, 1);
   GemmParams p = fp8_params(M, N, K, bn, inv_sa, inv_sb);
   p.off1 = s0; p.off2 = s0 + s1;
   GemmMaps tm;
@@ -847,7 +898,7 @@ extern "C" int tn_gemm_qkv_fp8(int mode, const void* A, int64_t lda, int a_e5m2,
     tm.b[1] = tm.b[2] = tm.b[0];
     for (int i = 0; i < 3; ++i)
       if ((rc = map_output(&tm.d[i], Ds[i], d_f32, uint64_t(seg[i]), uint64_t(N), ldd))) return rc;
-    return d_f32 ? launch_fp8<2>(a_e5m2, bn, tm, p, stream) : launch_fp8<0>(a_e5m2, bn, tm, p, stream);
+    return d_f32 ? launch_fp8<2>(op, bn, tm, p, stream) : launch_fp8<0>(op, bn, tm, p, stream);
   }
   if (mode == 0) {
     if (rope_cos) {
@@ -862,9 +913,84 @@ extern "C" int tn_gemm_qkv_fp8(int mode, const void* A, int64_t lda, int a_e5m2,
     for (int i = 0; i < 3; ++i)
       if ((rc = map_operand_fp8(&tm.b[i], Bs[i], uint64_t(N), uint64_t(seg[i]), ldb, bn))) return rc;
   }
-  TN_REQUIRE(!d_f32, "tn_gemm_qkv_fp8: modes 0 and 1 write bf16");
+  TN_REQUIRE(!d_f32, "%s: modes 0 and 1 write bf16", name);
   if ((rc = map_output(&tm.d[0], D0, 0, uint64_t(M), uint64_t(N), ldd))) return rc;
   tm.d[1] = tm.d[2] = tm.d[0];
-  return launch_fp8<0>(a_e5m2, bn, tm, p, stream);
+  return launch_fp8<0>(op, bn, tm, p, stream);
 }
+#undef TN_FP8_REQUIRE_VEC
 #undef TN_FP8_REQUIRE_COMMON
+
+extern "C" int tn_gemm_fp8(const void* A, int64_t lda, int a_e5m2, const void* B, int64_t ldb, void* D, int64_t ldd,
+                           int d_f32, const void* R, int64_t ldr, int M, int N, int K, const float* inv_sa,
+                           const float* inv_sb, tn_stream_t stream_) {
+  clear_error();
+  return gemm_fp8("tn_gemm_fp8", a_e5m2 ? 2 : 1, A, lda, B, ldb, D, ldd, d_f32, R, ldr, M, N, K, inv_sa, inv_sb,
+                  static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int tn_gemm_swiglu_fp8(const void* X, int64_t ldx, int x_e5m2, const void* Wg, const void* Wu, int64_t ldw,
+                                  void* G, void* U, void* H, int64_t ldh, int M, int N, int K, const float* inv_sx,
+                                  const float* inv_sw, tn_stream_t stream_) {
+  clear_error();
+  return gemm_swiglu_fp8("tn_gemm_swiglu_fp8", x_e5m2 ? 2 : 1, X, ldx, Wg, Wu, ldw, G, U, H, ldh, M, N, K, inv_sx,
+                         inv_sw, static_cast<cudaStream_t>(stream_));
+}
+
+// W is the K-major transposed copy of down_proj.weight: [N = ffn, K = d]
+extern "C" int tn_gemm_dswiglu_fp8(const void* dY, int64_t lddy, int dy_e5m2, const void* W, int64_t ldw, const void* G,
+                                   const void* U, int64_t ldgu, void* dG, void* dU, int64_t lddg, int M, int N, int K,
+                                   const float* inv_sa, const float* inv_sb, tn_stream_t stream_) {
+  clear_error();
+  return gemm_dswiglu_fp8("tn_gemm_dswiglu_fp8", dy_e5m2 ? 2 : 1, dY, lddy, W, ldw, G, U, ldgu, dG, dU, lddg, M, N, K,
+                          inv_sa, inv_sb, static_cast<cudaStream_t>(stream_));
+}
+
+// Modes as tn_gemm_qkv_bf16, all operands K-major: 1 = dgrad with B_i the [N, s_i] column blocks of Wᵀ (row stride
+// ldb), 2 = wgrad with A = the transposed gradient [s0+s1+s2, K] and B0 = the transposed layer input [N, K].
+extern "C" int tn_gemm_qkv_fp8(int mode, const void* A, int64_t lda, int a_e5m2, const void* B0, const void* B1,
+                               const void* B2, int64_t ldb, void* D0, void* D1, void* D2, int64_t ldd, int d_f32, int s0,
+                               int s1, int s2, int M, int N, int K, const void* rope_cos, const void* rope_sin,
+                               const float* inv_sa, const float* inv_sb, tn_stream_t stream_) {
+  clear_error();
+  const int op = a_e5m2 ? 2 : 1;
+  return gemm_qkv_fp8("tn_gemm_qkv_fp8", op, op, mode, A, lda, B0, B1, B2, ldb, D0, D1, D2, ldd, d_f32, s0, s1, s2, M,
+                      N, K, rope_cos, rope_sin, inv_sa, inv_sb, static_cast<cudaStream_t>(stream_));
+}
+
+// Rowwise: inv_sa [M] and inv_sb [N] (SwiGLU: inv_sw [2N], the gate rows then the up rows; QKV mode 0: inv_sb over the
+// rows of [Wq;Wk;Wv], N long).  `promoted` selects the separate fp32 accumulator (dgrad, wgrad); the dSwiGLU GEMM and
+// QKV modes 1 and 2 always promote, the SwiGLU GEMM and QKV mode 0 never do.
+extern "C" int tn_gemm_fp8_rowwise(const void* A, int64_t lda, const void* B, int64_t ldb, void* D, int64_t ldd,
+                                   int d_f32, const void* R, int64_t ldr, int M, int N, int K, const float* inv_sa,
+                                   const float* inv_sb, int promoted, tn_stream_t stream_) {
+  clear_error();
+  return gemm_fp8("tn_gemm_fp8_rowwise", promoted ? 4 : 3, A, lda, B, ldb, D, ldd, d_f32, R, ldr, M, N, K, inv_sa,
+                  inv_sb, static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int tn_gemm_swiglu_fp8_rowwise(const void* X, int64_t ldx, const void* Wg, const void* Wu, int64_t ldw,
+                                          void* G, void* U, void* H, int64_t ldh, int M, int N, int K,
+                                          const float* inv_sx, const float* inv_sw, tn_stream_t stream_) {
+  clear_error();
+  return gemm_swiglu_fp8("tn_gemm_swiglu_fp8_rowwise", 3, X, ldx, Wg, Wu, ldw, G, U, H, ldh, M, N, K, inv_sx, inv_sw,
+                         static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int tn_gemm_dswiglu_fp8_rowwise(const void* dY, int64_t lddy, const void* W, int64_t ldw, const void* G,
+                                           const void* U, int64_t ldgu, void* dG, void* dU, int64_t lddg, int M, int N,
+                                           int K, const float* inv_sa, const float* inv_sb, tn_stream_t stream_) {
+  clear_error();
+  return gemm_dswiglu_fp8("tn_gemm_dswiglu_fp8_rowwise", 4, dY, lddy, W, ldw, G, U, ldgu, dG, dU, lddg, M, N, K,
+                          inv_sa, inv_sb, static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int tn_gemm_qkv_fp8_rowwise(int mode, const void* A, int64_t lda, const void* B0, const void* B1,
+                                       const void* B2, int64_t ldb, void* D0, void* D1, void* D2, int64_t ldd, int d_f32,
+                                       int s0, int s1, int s2, int M, int N, int K, const void* rope_cos,
+                                       const void* rope_sin, const float* inv_sa, const float* inv_sb,
+                                       tn_stream_t stream_) {
+  clear_error();
+  return gemm_qkv_fp8("tn_gemm_qkv_fp8_rowwise", 3, 4, mode, A, lda, B0, B1, B2, ldb, D0, D1, D2, ldd, d_f32, s0, s1,
+                      s2, M, N, K, rope_cos, rope_sin, inv_sa, inv_sb, static_cast<cudaStream_t>(stream_));
+}

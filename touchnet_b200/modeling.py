@@ -151,14 +151,15 @@ class B200DecoderLayer(nn.Module):
         self.input_layernorm = B200RMSNorm(config.hidden_size, eps)
         self.post_attention_layernorm = B200RMSNorm(config.hidden_size, eps)
 
-    def forward(self, hidden_states, cos, sin, plan, fp8: bool = False):
+    def forward(self, hidden_states, cos, sin, plan, fp8: bool = False, float8_recipe_name: str = "tensorwise"):
         a, m = self.self_attn, self.mlp
         if plan.tp is None:
             return ops.decoder_layer(
                 hidden_states, self.input_layernorm.weight, a.q_proj.weight, a.k_proj.weight, a.v_proj.weight,
                 a.q_proj.bias, a.k_proj.bias, a.v_proj.bias, a.o_proj.weight, self.post_attention_layernorm.weight,
                 m.gate_proj.weight, m.up_proj.weight, m.down_proj.weight, cos, sin, plan, a.num_heads,
-                a.num_key_value_heads, self.input_layernorm.variance_epsilon, a.head_dim, fp8)
+                a.num_key_value_heads, self.input_layernorm.variance_epsilon, a.head_dim, fp8,
+                float8_recipe_name=float8_recipe_name)
         # tensor parallel (tensor_parallel.py): this rank's weight shards, H/tp and KV/tp heads
         from .tensor_parallel import local
         wq, wk = local(a.q_proj.weight), local(a.k_proj.weight)
@@ -167,7 +168,7 @@ class B200DecoderLayer(nn.Module):
             local(a.q_proj.bias), local(a.k_proj.bias), local(a.v_proj.bias), local(a.o_proj.weight),
             local(self.post_attention_layernorm.weight), local(m.gate_proj.weight), local(m.up_proj.weight),
             local(m.down_proj.weight), cos, sin, plan, wq.shape[0] // a.head_dim, wk.shape[0] // a.head_dim,
-            self.input_layernorm.variance_epsilon, fp8=fp8)
+            self.input_layernorm.variance_epsilon, fp8=fp8, float8_recipe_name=float8_recipe_name)
 
 
 class B200LlamaModel(nn.Module):
@@ -185,6 +186,8 @@ class B200LlamaModel(nn.Module):
         # FP8 projections in every decoder block (ops.block_forward); cached decoding stays bf16.  A plain attribute:
         # no parameter or buffer, so state dicts do not change
         self.float8_training = bool(_cfg(config, "float8_training", False))
+        # the FP8 recipe when float8_training is on: "tensorwise" (default) or "rowwise"
+        self.float8_recipe_name = ops.check_fp8_recipe(_cfg(config, "float8_recipe_name", "tensorwise"))
         hd = _cfg(config, "head_dim", config.hidden_size // config.num_attention_heads)
         if hd > 128 or hd % 8:
             raise TouchNetB200Error(f"touchnet_b200 attention kernels are built for head_dim 128 (smaller multiples of 8 run "
@@ -225,7 +228,7 @@ class B200LlamaModel(nn.Module):
         if x.dtype != torch.bfloat16:
             x = x.to(torch.bfloat16)
         for layer in self.layers:
-            x = layer(x, cos, sin, plan, self.float8_training)
+            x = layer(x, cos, sin, plan, self.float8_training, self.float8_recipe_name)
         return self.norm(x)
 
 
@@ -311,6 +314,16 @@ class B200LlamaForCausalLM(nn.Module):
     @float8_training.setter
     def float8_training(self, v: bool):
         self.model.float8_training = bool(v)
+
+    @property
+    def float8_recipe_name(self) -> str:
+        """The FP8 recipe of float8_training: "tensorwise" (torchao's default: one scale per tensor, e5m2 gradients) or
+        "rowwise" (one power-of-two scale per row, e4m3 throughout).  Set from the config key `float8_recipe_name`."""
+        return self.model.float8_recipe_name
+
+    @float8_recipe_name.setter
+    def float8_recipe_name(self, v: str):
+        self.model.float8_recipe_name = ops.check_fp8_recipe(v)
 
     # -- HF surface the reference touches -------------------------------------------------------------------
     def get_input_embeddings(self):
@@ -441,6 +454,8 @@ class B200TouchAudioForCausalLM(nn.Module):
         object.__setattr__(self.language_model, "_tn_fsdp_root", self)
         if getattr(config, "float8_training", None) is not None:   # the top-level key of the model JSON wins
             self.float8_training = config.float8_training
+        if getattr(config, "float8_recipe_name", None) is not None:
+            self.float8_recipe_name = config.float8_recipe_name
 
     @property
     def fused_linear_ce(self) -> bool:
@@ -457,6 +472,14 @@ class B200TouchAudioForCausalLM(nn.Module):
     @float8_training.setter
     def float8_training(self, v: bool):
         self.language_model.float8_training = bool(v)
+
+    @property
+    def float8_recipe_name(self) -> str:
+        return self.language_model.float8_recipe_name
+
+    @float8_recipe_name.setter
+    def float8_recipe_name(self, v: str):
+        self.language_model.float8_recipe_name = v
 
     @property
     def model(self):  # the reference's llama post_init / get_num_params reach `model.model.*`

@@ -382,6 +382,159 @@ def gemm_qkv_wgrad_fp8(dqkv_t, x_t, f32: bool, nq: int, nkv: int, inv_a, inv_b):
     return outs
 
 
+# Rowwise recipe (torchao's "rowwise"): every operand e4m3 with one power-of-two scale per row along the GEMM's reduction
+# axis; the 1/s vectors stay on the device.
+def _fp8_axis_input(x: torch.Tensor) -> None:
+    """A bf16 [rows, cols] view with unit inner stride.  These checks come before the device checks of the callers."""
+    if x.dtype != BF16 or x.dim() != 2 or x.stride(1) != 1:
+        raise _lib.TouchNetB200Error(f"x must be a 2-D bfloat16 view with unit inner stride, got {x.dtype} "
+                                     f"{tuple(x.shape)} strides {tuple(x.stride())}")
+
+
+def _fp8_vec(v: torch.Tensor, n: int, name: str) -> None:
+    """A contiguous float32 vector of n entries (amaxes or 1/s)."""
+    if v.dtype != torch.float32 or v.dim() != 1 or v.numel() != n or not v.is_contiguous():
+        raise _lib.TouchNetB200Error(f"{name} must be a contiguous float32 vector of {n}, got {v.dtype} "
+                                     f"{tuple(v.shape)}")
+
+
+def _fp8_copy(t: torch.Tensor, shape, name: str) -> None:
+    """An e4m3 output [rows, cols] (a column block of a wider buffer is fine) with unit inner stride."""
+    if t.dtype != F8E4M3 or tuple(t.shape) != tuple(shape) or t.stride(1) != 1:
+        raise _lib.TouchNetB200Error(f"{name} must be float8_e4m3fn {tuple(shape)} with unit inner stride, got "
+                                     f"{t.dtype} {tuple(t.shape)}")
+
+
+def fp8_rowwise_cast(x: torch.Tensor, out=None, inv=None):
+    """The e4m3 row-major copy of bf16 x [rows, cols], one scale per row; returns (copy, 1/s [rows])."""
+    _fp8_axis_input(x)
+    rows, cols = x.shape
+    out = torch.empty((rows, cols), dtype=F8E4M3, device=x.device) if out is None else out
+    inv = torch.empty(rows, dtype=torch.float32, device=x.device) if inv is None else inv
+    _fp8_copy(out, (rows, cols), "out")
+    _fp8_vec(inv, rows, "inv")
+    for t, n in ((x, "x"), (out, "out"), (inv, "inv")):
+        _chk(t, n)
+    _lib.call("tn_fp8_rowwise_cast_bf16", x.data_ptr(), x.stride(0), rows, cols, out.data_ptr(), out.stride(0),
+              inv.data_ptr(), _st())
+    return out, inv
+
+
+def fp8_colwise_amax(x: torch.Tensor, amax: torch.Tensor) -> None:
+    """amax[c] = max(amax[c], max_r |x[r, c]|) over bf16 x [rows, cols]; `amax` [cols] is zeroed by the caller."""
+    _fp8_axis_input(x)
+    _fp8_vec(amax, x.shape[1], "amax")
+    _chk(x, "x"); _chk(amax, "amax")
+    _lib.call("tn_fp8_colwise_amax_bf16", x.data_ptr(), x.stride(0), x.shape[0], x.shape[1], amax.data_ptr(), _st())
+
+
+def fp8_colwise_cast_t(x: torch.Tensor, amax: torch.Tensor, out_t=None, inv=None):
+    """The e4m3 transposed copy [cols, rows] of bf16 x, one scale per column of x from `amax` [cols]; returns
+    (copy, 1/s [cols])."""
+    _fp8_axis_input(x)
+    rows, cols = x.shape
+    _fp8_vec(amax, cols, "amax")
+    out_t = torch.empty((cols, rows), dtype=F8E4M3, device=x.device) if out_t is None else out_t
+    inv = torch.empty(cols, dtype=torch.float32, device=x.device) if inv is None else inv
+    _fp8_copy(out_t, (cols, rows), "out_t")
+    _fp8_vec(inv, cols, "inv")
+    for t, n in ((x, "x"), (amax, "amax"), (out_t, "out_t"), (inv, "inv")):
+        _chk(t, n)
+    _lib.call("tn_fp8_colwise_cast_t_bf16", x.data_ptr(), x.stride(0), rows, cols, amax.data_ptr(), out_t.data_ptr(),
+              out_t.stride(0), inv.data_ptr(), _st())
+    return out_t, inv
+
+
+def _fp8_rowwise_operands(a: torch.Tensor, b: torch.Tensor) -> None:
+    if a.dtype != F8E4M3 or b.dtype != F8E4M3:
+        raise _lib.TouchNetB200Error(f"both operands of a rowwise FP8 GEMM are float8_e4m3fn, got {a.dtype} and {b.dtype}")
+    _chk(a, "a"); _chk(b, "b")
+    assert a.dim() == 2 and b.dim() == 2 and a.stride(1) == 1 and b.stride(1) == 1
+
+
+def gemm_fp8_rowwise(a, b, inv_a, inv_b, *, promoted: bool, out_f32: bool = False, residual=None, out=None):
+    """D[M,N] = a[M,K]·b[N,K]ᵀ · inv_a[m] · inv_b[n] (+R): e4m3 operands, 1/s vectors over the rows of a and b.
+    `promoted`: per-stage partial sums in a separate fp32 accumulator (dgrad, wgrad)."""
+    _fp8_rowwise_operands(a, b)
+    (M, K), N = a.shape, b.shape[0]
+    assert b.shape[1] == K and inv_a.numel() == M and inv_b.numel() == N, (a.shape, b.shape)
+    dt = torch.float32 if out_f32 else BF16
+    if out is None:
+        out = torch.empty((M, N), dtype=dt, device=a.device)
+    _lib.call("tn_gemm_fp8_rowwise", a.data_ptr(), a.stride(0), b.data_ptr(), b.stride(0), out.data_ptr(), out.stride(0),
+              int(out_f32), _lib.ptr(residual), 0 if residual is None else residual.stride(0), M, N, K, inv_a.data_ptr(),
+              inv_b.data_ptr(), int(promoted), _st())
+    return out
+
+
+def gemm_swiglu_fp8_rowwise(x, wg, wu, inv_x, inv_w, need_gu: bool = True):
+    """gemm_swiglu on e4m3 x [M,K] and wg / wu [N,K]; inv_w [2N] holds the 1/s of the gate rows, then the up rows."""
+    _fp8_rowwise_operands(x, wg)
+    _fp8_rowwise_operands(x, wu)
+    M, K = x.shape
+    N = wg.shape[0]
+    assert wg.shape == wu.shape == (N, K) and wg.stride(0) == wu.stride(0) and inv_w.numel() == 2 * N
+    h = torch.empty((M, N), dtype=BF16, device=x.device)
+    g = torch.empty_like(h) if need_gu else None
+    u = torch.empty_like(h) if need_gu else None
+    _lib.call("tn_gemm_swiglu_fp8_rowwise", x.data_ptr(), x.stride(0), wg.data_ptr(), wu.data_ptr(), wg.stride(0),
+              _lib.ptr(g), _lib.ptr(u), h.data_ptr(), N, M, N, K, inv_x.data_ptr(), inv_w.data_ptr(), _st())
+    return g, u, h
+
+
+def gemm_dswiglu_fp8_rowwise(dy, wd_t, g, u, inv_a, inv_b):
+    """gemm_dswiglu_fp8 with rowwise scales (promoted accumulation)."""
+    _fp8_rowwise_operands(dy, wd_t)
+    M, K = dy.shape
+    N = wd_t.shape[0]
+    if not (_FUSE_DSWIGLU and M >= 256 and N >= 256 and g.stride(0) == u.stride(0)):
+        return swiglu_bwd(g, u, gemm_fp8_rowwise(dy, wd_t, inv_a, inv_b, promoted=True))
+    dg = torch.empty_like(g)
+    du = torch.empty_like(u)
+    _lib.call("tn_gemm_dswiglu_fp8_rowwise", dy.data_ptr(), dy.stride(0), wd_t.data_ptr(), wd_t.stride(0), g.data_ptr(),
+              u.data_ptr(), g.stride(0), dg.data_ptr(), du.data_ptr(), dg.stride(0), M, N, K, inv_a.data_ptr(),
+              inv_b.data_ptr(), _st())
+    return dg, du
+
+
+def gemm_qkv_fwd_fp8_rowwise(x, wq, wk, wv, inv_x, inv_w, rope=None):
+    """gemm_qkv_fwd on e4m3 x [M,K] and wq / wk / wv [n_i, K]; inv_w: the 1/s of the rows of [Wq;Wk;Wv]."""
+    _fp8_rowwise_operands(x, wq)
+    M, K = x.shape
+    nq, nkv = wq.shape[0], wk.shape[0]
+    out = torch.empty((M, nq + 2 * nkv), dtype=BF16, device=x.device)
+    _lib.call("tn_gemm_qkv_fp8_rowwise", 0, x.data_ptr(), x.stride(0), wq.data_ptr(), wk.data_ptr(), wv.data_ptr(),
+              wq.stride(0), out.data_ptr(), None, None, out.stride(0), 0, nq, nkv, nkv, M, nq + 2 * nkv, K,
+              None if rope is None else rope[0].data_ptr(), None if rope is None else rope[1].data_ptr(),
+              inv_x.data_ptr(), inv_w.data_ptr(), _st())
+    return out
+
+
+def gemm_qkv_dgrad_fp8_rowwise(dqkv, w_t, nq: int, nkv: int, inv_a, inv_b):
+    """gemm_qkv_dgrad_fp8 with rowwise scales: inv_a over the rows of dqkv, inv_b over the rows of w_t."""
+    _fp8_rowwise_operands(dqkv, w_t)
+    M, Kt = dqkv.shape
+    d = w_t.shape[0]
+    out = torch.empty((M, d), dtype=BF16, device=dqkv.device)
+    _lib.call("tn_gemm_qkv_fp8_rowwise", 1, dqkv.data_ptr(), dqkv.stride(0), w_t.data_ptr(), w_t[:, nq:].data_ptr(),
+              w_t[:, nq + nkv:].data_ptr(), w_t.stride(0), out.data_ptr(), None, None, out.stride(0), 0, nq, nkv, nkv,
+              M, d, Kt, None, None, inv_a.data_ptr(), inv_b.data_ptr(), _st())
+    return out
+
+
+def gemm_qkv_wgrad_fp8_rowwise(dqkv_t, x_t, f32: bool, nq: int, nkv: int, inv_a, inv_b):
+    """gemm_qkv_wgrad_fp8 with rowwise scales: inv_a over the rows of dqkv_t, inv_b over the rows of x_t."""
+    _fp8_rowwise_operands(dqkv_t, x_t)
+    Mt, Mred = dqkv_t.shape
+    d = x_t.shape[0]
+    dt = torch.float32 if f32 else BF16
+    outs = [torch.empty((n, d), dtype=dt, device=x_t.device) for n in (nq, nkv, nkv)]
+    _lib.call("tn_gemm_qkv_fp8_rowwise", 2, dqkv_t.data_ptr(), dqkv_t.stride(0), x_t.data_ptr(), None, None,
+              x_t.stride(0), outs[0].data_ptr(), outs[1].data_ptr(), outs[2].data_ptr(), d, int(f32), nq, nkv, nkv, Mt,
+              d, Mred, None, None, inv_a.data_ptr(), inv_b.data_ptr(), _st())
+    return outs
+
+
 def _fp8_quant(xs, st, slot: int, e5m2: bool, row: bool = True, t: bool = True):
     """Quantise the bf16 tensors `xs` with one dynamic scale, the amax over all of them, kept in row `slot` of the
     device scale table st [n, 2] = (amax, 1/s).  Returns [(row-major, transposed)] per tensor."""
@@ -820,7 +973,7 @@ def _unpad_heads(x: torch.Tensor, heads: int, hd: int) -> torch.Tensor:
 
 
 def block_forward(x2, ln1, wqb, wkb, wvb, bq, bk, bv, wob, ln2, wgb, wub, wdb, cos, sin, H, KV, eps, hd, attend, tp=None,
-                  need_gu=True, qkv_rows=None, fp8: bool = False):
+                  need_gu=True, qkv_rows=None, fp8: bool = False, fp8_recipe: str = "tensorwise"):
     """Forward of one pre-norm decoder block on rows x2 [M, d] with bf16 working weights - the body shared by training
     (DecoderLayerFn), prompt prefill and cached decoding (generation.py), which differ only in `attend(q, k, v) ->
     (o, lse, k, v)`: q/k/v arrive projected, rotated and (head_dim < 128) zero-padded to 128-wide heads.
@@ -829,10 +982,11 @@ def block_forward(x2, ln1, wqb, wkb, wvb, bq, bk, bv, wob, ln2, wgb, wub, wdb, c
     Returns (out, saved) with saved = (rstd1, h1, q, k, v, o, lse, x1, rstd2, h2, g, u, hm) for the backward.
     fp8=True (training only, no tensor parallelism): the seven projections run as FP8 GEMMs on dynamically scaled e4m3
     copies of their inputs and weights; h1, h2 and hm in `saved` are then the transposed e4m3 copies the weight
-    gradients need, and saved ends with (oᵀ in e4m3, the scale table)."""
+    gradients need, and saved ends with (oᵀ in e4m3, the recipe's saved scales).  `fp8_recipe`: "tensorwise" (one
+    scale per tensor, e5m2 gradients) or "rowwise" (per-row power-of-two scales, e4m3 throughout)."""
     if fp8:
         return _block_forward_fp8(x2, ln1, wqb, wkb, wvb, bq, bk, bv, wob, ln2, wgb, wub, wdb, cos, sin, H, KV, eps, hd,
-                                  attend)
+                                  attend, fp8_recipe)
     h1, _, rstd1 = rmsnorm_fwd(x2, ln1, eps)
     if tp is not None:
         h1 = tp.gather_rows(h1, keep=True)                               # [B*T, d]: every row, for the local heads
@@ -867,23 +1021,194 @@ def block_forward(x2, ln1, wqb, wkb, wvb, bq, bk, bv, wob, ln2, wgb, wub, wdb, c
     return out, (rstd1, h1, q, k, v, o, lse, x1, rstd2, h2, g, u, hm)
 
 
-def _block_forward_fp8(x2, ln1, wqb, wkb, wvb, bq, bk, bv, wob, ln2, wgb, wub, wdb, cos, sin, H, KV, eps, hd, attend):
-    """block_forward with FP8 projections (see there).  q/k/v weights share one scale, as do gate/up: the fused QKV
-    dgrad sums over the three stacked weights and the SwiGLU tile holds gate and up rows, so one post-accumulation
-    scale must cover them."""
+FP8_RECIPES = ("tensorwise", "rowwise")
+
+
+def check_fp8_recipe(name: str) -> str:
+    """The recipe names the FP8 block accepts (the model config key `float8_recipe_name`)."""
+    if name not in FP8_RECIPES:
+        raise _lib.TouchNetB200Error(f"float8_recipe_name must be 'tensorwise' or 'rowwise', got {name!r}")
+    return name
+
+
+def _seg(inv, off: int, n: int):
+    """The 1/s of rows [off, off + n) of a quantised operand: a per-tensor scale covers them all."""
+    return inv if inv.dim() == 0 else inv[off:off + n]
+
+
+class _Tensorwise:
+    """torchao's tensorwise recipe: one dynamic scale per tensor, e4m3 activations and weights, e5m2 gradients.  The
+    q/k/v weights share one scale, as do gate/up, and dq|dk|dv: the fused QKV dgrad sums over the three stacked weights
+    and the SwiGLU tile holds gate and up rows, so one post-accumulation scale must cover them.  The forward's scale
+    table [8, 2] = (amax, 1/s) is saved; the backward re-quantises the transposed weights at its amaxes."""
+
+    def __init__(self, dev, dims, saved=None):
+        self.fwd = torch.zeros((8, 2), dtype=torch.float32, device=dev) if saved is None else saved
+        self.bwd = None if saved is None else torch.zeros((5, 2), dtype=torch.float32, device=dev)
+        self.state = self.fwd
+
+    def act(self, x, slot):
+        """(row-major copy, 1/s, transposed copy, 1/s) of a forward activation."""
+        ((x8, x_t),) = _fp8_quant([x], self.fwd, slot, False)
+        return x8, self.fwd[slot, 1], x_t, self.fwd[slot, 1]
+
+    def grad(self, dy, slot):
+        ((d8, d_t),) = _fp8_quant([dy], self.bwd, slot, True)
+        return d8, self.bwd[slot, 1], d_t, self.bwd[slot, 1]
+
+    def saved_inv(self, slot):
+        return self.fwd[slot, 1]
+
+    def weights(self, ws, slot):
+        """Row-major copies of a weight group; returns (copies, 1/s of each, 1/s of the stacked group)."""
+        inv = self.fwd[slot, 1]
+        return [w for w, _ in _fp8_quant(ws, self.fwd, slot, False, t=False)], [inv] * len(ws), inv
+
+    def weight_t(self, ws, slot):
+        """The transposed copy [in, Σ out] of the stacked group and its 1/s."""
+        if len(ws) == 1:
+            return _fp8_weight_t(ws[0], self.fwd, slot), self.fwd[slot, 1]
+        w_t = torch.empty((ws[0].shape[1], sum(w.shape[0] for w in ws)), dtype=F8E4M3, device=ws[0].device)
+        off = 0
+        for w in ws:
+            _fp8_weight_t(w, self.fwd, slot, out_t=w_t[:, off:off + w.shape[0]])
+            off += w.shape[0]
+        return w_t, self.fwd[slot, 1]
+
+    def qkv_grad(self, dys, slot):
+        """(dq|dk|dv row-major, 1/s, transposed, 1/s) with one scale over the three."""
+        M, tot, dev = dys[0].shape[0], sum(dy.shape[1] for dy in dys), dys[0].device
+        d8 = torch.empty((M, tot), dtype=F8E5M2, device=dev)
+        d_t = torch.empty((tot, M), dtype=F8E5M2, device=dev)
+        for dy in dys:
+            fp8_amax(dy, self.bwd[slot, 0])
+        off = 0
+        for dy in dys:
+            n = dy.shape[1]
+            fp8_cast(dy, self.bwd[slot, 0], True, inv=self.bwd[slot, 1], out=d8[:, off:off + n], out_t=d_t[off:off + n])
+            off += n
+        return d8, self.bwd[slot, 1], d_t, self.bwd[slot, 1]
+
+    def gemm(self, a, b, inv_a, inv_b, **kw):
+        return gemm_fp8(a, b, inv_a, inv_b, **kw)
+
+    def swiglu(self, x, wg, wu, inv_x, inv_w):
+        return gemm_swiglu_fp8(x, wg, wu, inv_x, inv_w)
+
+    def dswiglu(self, dy, wd_t, g, u, inv_a, inv_b):
+        return gemm_dswiglu_fp8(dy, wd_t, g, u, inv_a, inv_b)
+
+    def qkv_fwd(self, x, wq, wk, wv, inv_x, inv_w, rope):
+        return gemm_qkv_fwd_fp8(x, wq, wk, wv, inv_x, inv_w, rope=rope)
+
+    def qkv_dgrad(self, dqkv, w_t, nq, nkv, inv_a, inv_b):
+        return gemm_qkv_dgrad_fp8(dqkv, w_t, nq, nkv, inv_a, inv_b)
+
+    def qkv_wgrad(self, dqkv_t, x_t, f32, nq, nkv, inv_a, inv_b):
+        return gemm_qkv_wgrad_fp8(dqkv_t, x_t, f32, nq, nkv, inv_a, inv_b)
+
+
+class _Rowwise:
+    """torchao's rowwise recipe: every operand e4m3, one power-of-two scale per row along the GEMM's reduction axis.
+    Activations and gradients get a row-scaled copy and a column-scaled transposed copy (for wgrad), weights a
+    row-scaled copy (forward) and a column-scaled transposed one (dgrad).  dq|dk|dv share each row's scale, and the
+    transposed [Wq;Wk;Wv] each column's, because the fused QKV dgrad sums over the stacked rows.  The forward saves the
+    1/s of its transposed copies (h1, o, h2, hm) in one vector; forward GEMMs accumulate in the tensor-core accumulator,
+    backward GEMMs promote."""
+
+    def __init__(self, dev, dims, saved=None):
+        d, n_o, ffn = dims
+        off, self.t_off = 0, {}
+        for slot, n in ((_F8_H1, d), (_F8_O, n_o), (_F8_H2, d), (_F8_HM, ffn)):
+            self.t_off[slot] = (off, n)
+            off += n
+        self.state = torch.empty(off, dtype=torch.float32, device=dev) if saved is None else saved
+        self.promoted = saved is not None
+
+    def saved_inv(self, slot):
+        off, n = self.t_off[slot]
+        return self.state[off:off + n]
+
+    def _quant(self, x, inv_t=None):
+        x8, inv = fp8_rowwise_cast(x)
+        amax = torch.zeros(x.shape[1], dtype=torch.float32, device=x.device)
+        fp8_colwise_amax(x, amax)
+        x_t, inv_t = fp8_colwise_cast_t(x, amax, inv=inv_t)
+        return x8, inv, x_t, inv_t
+
+    def act(self, x, slot):
+        return self._quant(x, self.saved_inv(slot))
+
+    def grad(self, dy, slot):
+        return self._quant(dy)
+
+    def weights(self, ws, slot):
+        inv = torch.empty(sum(w.shape[0] for w in ws), dtype=torch.float32, device=ws[0].device)
+        w8s, invs, off = [], [], 0
+        for w in ws:
+            n = w.shape[0]
+            w8s.append(fp8_rowwise_cast(w, inv=inv[off:off + n])[0])
+            invs.append(inv[off:off + n])
+            off += n
+        return w8s, invs, inv
+
+    def weight_t(self, ws, slot):
+        dev, d = ws[0].device, ws[0].shape[1]
+        amax = torch.zeros(d, dtype=torch.float32, device=dev)
+        for w in ws:
+            fp8_colwise_amax(w, amax)
+        w_t = torch.empty((d, sum(w.shape[0] for w in ws)), dtype=F8E4M3, device=dev)
+        inv = torch.empty(d, dtype=torch.float32, device=dev)
+        off = 0
+        for w in ws:
+            fp8_colwise_cast_t(w, amax, out_t=w_t[:, off:off + w.shape[0]], inv=inv)
+            off += w.shape[0]
+        return w_t, inv
+
+    def qkv_grad(self, dys, slot):
+        return self._quant(torch.cat(dys, dim=1))
+
+    def gemm(self, a, b, inv_a, inv_b, **kw):
+        return gemm_fp8_rowwise(a, b, inv_a, inv_b, promoted=self.promoted, **kw)
+
+    def swiglu(self, x, wg, wu, inv_x, inv_w):
+        return gemm_swiglu_fp8_rowwise(x, wg, wu, inv_x, inv_w)
+
+    def dswiglu(self, dy, wd_t, g, u, inv_a, inv_b):
+        return gemm_dswiglu_fp8_rowwise(dy, wd_t, g, u, inv_a, inv_b)
+
+    def qkv_fwd(self, x, wq, wk, wv, inv_x, inv_w, rope):
+        return gemm_qkv_fwd_fp8_rowwise(x, wq, wk, wv, inv_x, inv_w, rope=rope)
+
+    def qkv_dgrad(self, dqkv, w_t, nq, nkv, inv_a, inv_b):
+        return gemm_qkv_dgrad_fp8_rowwise(dqkv, w_t, nq, nkv, inv_a, inv_b)
+
+    def qkv_wgrad(self, dqkv_t, x_t, f32, nq, nkv, inv_a, inv_b):
+        return gemm_qkv_wgrad_fp8_rowwise(dqkv_t, x_t, f32, nq, nkv, inv_a, inv_b)
+
+
+_FP8_RECIPE_CLASSES = {"tensorwise": _Tensorwise, "rowwise": _Rowwise}
+
+
+def _fp8_recipe(name, dev, wqb, wob, wgb, saved=None):
+    return _FP8_RECIPE_CLASSES[check_fp8_recipe(name)](dev, (wqb.shape[1], wob.shape[1], wgb.shape[0]), saved)
+
+
+def _block_forward_fp8(x2, ln1, wqb, wkb, wvb, bq, bk, bv, wob, ln2, wgb, wub, wdb, cos, sin, H, KV, eps, hd, attend,
+                       recipe="tensorwise"):
+    """block_forward with FP8 projections (see there) under `recipe` (_Tensorwise, _Rowwise)."""
     nq, nkv, d, ffn = wqb.shape[0], wkb.shape[0], wqb.shape[1], wgb.shape[0]
     _fp8_dims(x2.shape[0], d, nq, nkv, wob.shape[1], ffn)
-    st = torch.zeros((8, 2), dtype=torch.float32, device=x2.device)
-    inv = st[:, 1]
+    rc = _fp8_recipe(recipe, x2.device, wqb, wob, wgb)
     h1, _, rstd1 = rmsnorm_fwd(x2, ln1, eps)
-    ((h1_8, h1_t),) = _fp8_quant([h1], st, _F8_H1, False)
-    wq8, wk8, wv8 = (w for w, _ in _fp8_quant([wqb, wkb, wvb], st, _F8_WQKV, False, t=False))
+    h1_8, ih1, h1_t, _ = rc.act(h1, _F8_H1)
+    wqkv8, iwqkv, iwqkv_all = rc.weights([wqb, wkb, wvb], _F8_WQKV)
     rope_in_gemm = qkv_fusable(h1.shape[0], nq, nkv) and bq is None and hd == 128
     if qkv_fusable(h1.shape[0], nq, nkv):
-        qkv = gemm_qkv_fwd_fp8(h1_8, wq8, wk8, wv8, inv[_F8_H1], inv[_F8_WQKV], rope=(cos, sin) if rope_in_gemm else None)
+        qkv = rc.qkv_fwd(h1_8, *wqkv8, ih1, iwqkv_all, (cos, sin) if rope_in_gemm else None)
         q, k, v = qkv[:, :nq], qkv[:, nq:nq + nkv], qkv[:, nq + nkv:]
     else:
-        q, k, v = (gemm_fp8(h1_8, w8, inv[_F8_H1], inv[_F8_WQKV]) for w8 in (wq8, wk8, wv8))
+        q, k, v = (rc.gemm(h1_8, w8, ih1, iw) for w8, iw in zip(wqkv8, iwqkv))
     if bq is not None:
         q += bq.to(BF16); k += bk.to(BF16); v += bv.to(BF16)
     if not rope_in_gemm:
@@ -892,17 +1217,17 @@ def _block_forward_fp8(x2, ln1, wqb, wkb, wvb, bq, bk, bv, wob, ln2, wgb, wub, w
     if hd != 128:
         q, k, v = _pad_heads(q, H, hd), _pad_heads(k, KV, hd), _pad_heads(v, KV, hd)
     o, lse, k, v = attend(q, k, v)
-    ((o8, o_t),) = _fp8_quant([o if hd == 128 else _unpad_heads(o, H, hd)], st, _F8_O, False)
-    ((wo8, _),) = _fp8_quant([wob], st, _F8_WO, False, t=False)
-    x1 = gemm_fp8(o8, wo8, inv[_F8_O], inv[_F8_WO], residual=x2)
+    o8, io, o_t, _ = rc.act(o if hd == 128 else _unpad_heads(o, H, hd), _F8_O)
+    (wo8,), (iwo,), _ = rc.weights([wob], _F8_WO)
+    x1 = rc.gemm(o8, wo8, io, iwo, residual=x2)
     h2, _, rstd2 = rmsnorm_fwd(x1, ln2, eps)
-    ((h2_8, h2_t),) = _fp8_quant([h2], st, _F8_H2, False)
-    wg8, wu8 = (w for w, _ in _fp8_quant([wgb, wub], st, _F8_WGU, False, t=False))
-    g, u, hm = gemm_swiglu_fp8(h2_8, wg8, wu8, inv[_F8_H2], inv[_F8_WGU])
-    ((hm8, hm_t),) = _fp8_quant([hm], st, _F8_HM, False)
-    ((wd8, _),) = _fp8_quant([wdb], st, _F8_WD, False, t=False)
-    out = gemm_fp8(hm8, wd8, inv[_F8_HM], inv[_F8_WD], residual=x1)
-    return out, (rstd1, h1_t, q, k, v, o, lse, x1, rstd2, h2_t, g, u, hm_t, o_t, st)
+    h2_8, ih2, h2_t, _ = rc.act(h2, _F8_H2)
+    (wg8, wu8), _, iwgu = rc.weights([wgb, wub], _F8_WGU)
+    g, u, hm = rc.swiglu(h2_8, wg8, wu8, ih2, iwgu)
+    hm8, ihm, hm_t, _ = rc.act(hm, _F8_HM)
+    (wd8,), (iwd,), _ = rc.weights([wdb], _F8_WD)
+    out = rc.gemm(hm8, wd8, ihm, iwd, residual=x1)
+    return out, (rstd1, h1_t, q, k, v, o, lse, x1, rstd2, h2_t, g, u, hm_t, o_t, rc.state)
 
 
 def _fp8_weight_t(wb, st, slot, out_t=None):
@@ -911,34 +1236,36 @@ def _fp8_weight_t(wb, st, slot, out_t=None):
 
 
 def _block_backward_fp8(ctx, saved, d2):
-    """Weight and input gradients of the FP8 block: every incoming gradient is quantised to e5m2 (one scale for dq|dk|dv,
-    which the fused QKV dgrad sums over), dgrad = dY·Wᵀ and wgrad = dYᵀ·Xᵀ as FP8 GEMMs on K-major copies."""
+    """Weight and input gradients of the FP8 block under ctx.fp8_recipe: every incoming gradient is quantised (dq|dk|dv
+    as one operand, which the fused QKV dgrad sums over), dgrad = dY·Wᵀ and wgrad = dYᵀ·Xᵀ as FP8 GEMMs on K-major
+    copies."""
     (x2, ln1, ln2, wqb, wkb, wvb, wob, wgb, wub, wdb, cos, sin, rstd1, h1_t, q, k, v, o, lse, x1, rstd2, h2_t, g, u,
-     hm_t, o_t, st) = saved
+     hm_t, o_t, state) = saved
     H, KV, f32, hd = ctx.H, ctx.KV, ctx.f32, ctx.hd
-    M, dev = d2.shape[0], d2.device
-    inv = st[:, 1]
-    sb = torch.zeros((5, 2), dtype=torch.float32, device=dev)
-    ib = sb[:, 1]
+    rb = _fp8_recipe(ctx.fp8_recipe, d2.device, wqb, wob, wgb, saved=state)
     # ---- MLP ----
-    ((d2_8, d2_t),) = _fp8_quant([d2], sb, _F8_D2, True)
-    dg, du = gemm_dswiglu_fp8(d2_8, _fp8_weight_t(wdb, st, _F8_WD), g, u, ib[_F8_D2], inv[_F8_WD])
-    dwd = gemm_fp8(d2_t, hm_t, ib[_F8_D2], inv[_F8_HM], out_f32=f32)
-    del d2_8, d2_t
-    ((dg8, dg_t),) = _fp8_quant([dg], sb, _F8_DG, True)
-    ((du8, du_t),) = _fp8_quant([du], sb, _F8_DU, True)
+    d2_8, id2, d2_t, id2_t = rb.grad(d2, _F8_D2)
+    wd_t, iwd_t = rb.weight_t([wdb], _F8_WD)
+    dg, du = rb.dswiglu(d2_8, wd_t, g, u, id2, iwd_t)
+    dwd = rb.gemm(d2_t, hm_t, id2_t, rb.saved_inv(_F8_HM), out_f32=f32)
+    del d2_8, d2_t, wd_t
+    dg8, idg, dg_t, idg_t = rb.grad(dg, _F8_DG)
+    du8, idu, du_t, idu_t = rb.grad(du, _F8_DU)
     del dg, du
-    dh2 = gemm_fp8(dg8, _fp8_weight_t(wgb, st, _F8_WGU), ib[_F8_DG], inv[_F8_WGU])
-    dh2 = gemm_fp8(du8, _fp8_weight_t(wub, st, _F8_WGU), ib[_F8_DU], inv[_F8_WGU], residual=dh2, out=dh2)
-    dwg = gemm_fp8(dg_t, h2_t, ib[_F8_DG], inv[_F8_H2], out_f32=f32)
-    dwu = gemm_fp8(du_t, h2_t, ib[_F8_DU], inv[_F8_H2], out_f32=f32)
-    del dg8, dg_t, du8, du_t
+    wg_t, iwg_t = rb.weight_t([wgb], _F8_WGU)
+    dh2 = rb.gemm(dg8, wg_t, idg, iwg_t)
+    wu_t, iwu_t = rb.weight_t([wub], _F8_WGU)
+    dh2 = rb.gemm(du8, wu_t, idu, iwu_t, residual=dh2, out=dh2)
+    dwg = rb.gemm(dg_t, h2_t, idg_t, rb.saved_inv(_F8_H2), out_f32=f32)
+    dwu = rb.gemm(du_t, h2_t, idu_t, rb.saved_inv(_F8_H2), out_f32=f32)
+    del dg8, dg_t, du8, du_t, wg_t, wu_t
     dx1, dln2 = rmsnorm_bwd(x1, dh2, ln2, rstd2, ds_extra=d2)
     # ---- attention ----
-    ((dx1_8, dx1_t),) = _fp8_quant([dx1], sb, _F8_DX1, True)
-    do = gemm_fp8(dx1_8, _fp8_weight_t(wob, st, _F8_WO), ib[_F8_DX1], inv[_F8_WO])
-    dwo = gemm_fp8(dx1_t, o_t, ib[_F8_DX1], inv[_F8_O], out_f32=f32)
-    del dx1_8, dx1_t
+    dx1_8, idx1, dx1_t, idx1_t = rb.grad(dx1, _F8_DX1)
+    wo_t, iwo_t = rb.weight_t([wob], _F8_WO)
+    do = rb.gemm(dx1_8, wo_t, idx1, iwo_t)
+    dwo = rb.gemm(dx1_t, o_t, idx1_t, rb.saved_inv(_F8_O), out_f32=f32)
+    del dx1_8, dx1_t, wo_t
     if hd != 128:   # padded heads: gradients of the padded tensors, un-padded, then the inverse rotation at head_dim hd
         dq, dk, dv = attn_bwd(q, k, v, o, _pad_heads(do, H, hd), lse, ctx.plan, H, KV, ctx.scale)
         dq, dk, dv = _unpad_heads(dq, H, hd), _unpad_heads(dk, KV, hd), _unpad_heads(dv, KV, hd)
@@ -948,25 +1275,18 @@ def _block_backward_fp8(ctx, saved, d2):
         dq, dk, dv = attn_bwd(q, k, v, o, do, lse, ctx.plan, H, KV, ctx.scale, rope=(cos, sin))
     del do
     nq, nkv = wqb.shape[0], wkb.shape[0]
-    tot, offs, widths = nq + 2 * nkv, (0, nq, nq + nkv), (nq, nkv, nkv)
-    dqkv8 = torch.empty((M, tot), dtype=F8E5M2, device=dev)
-    dqkv_t = torch.empty((tot, M), dtype=F8E5M2, device=dev)
-    for dy in (dq, dk, dv):
-        fp8_amax(dy, sb[_F8_DQKV, 0])
-    for dy, off, n in zip((dq, dk, dv), offs, widths):
-        fp8_cast(dy, sb[_F8_DQKV, 0], True, inv=ib[_F8_DQKV], out=dqkv8[:, off:off + n], out_t=dqkv_t[off:off + n])
-    w_t = torch.empty((wqb.shape[1], tot), dtype=F8E4M3, device=dev)   # [Wq;Wk;Wv]ᵀ
-    for wb, off, n in zip((wqb, wkb, wvb), offs, widths):
-        _fp8_weight_t(wb, st, _F8_WQKV, out_t=w_t[:, off:off + n])
+    M = d2.shape[0]
+    dqkv8, idqkv, dqkv_t, idqkv_t = rb.qkv_grad((dq, dk, dv), _F8_DQKV)
+    w_t, iw_t = rb.weight_t([wqb, wkb, wvb], _F8_WQKV)   # [Wq;Wk;Wv]ᵀ
     if qkv_fusable(M, nq, nkv):
-        dh1 = gemm_qkv_dgrad_fp8(dqkv8, w_t, nq, nkv, ib[_F8_DQKV], inv[_F8_WQKV])
-        dwq, dwk, dwv = gemm_qkv_wgrad_fp8(dqkv_t, h1_t, f32, nq, nkv, ib[_F8_DQKV], inv[_F8_H1])
+        dh1 = rb.qkv_dgrad(dqkv8, w_t, nq, nkv, idqkv, iw_t)
+        dwq, dwk, dwv = rb.qkv_wgrad(dqkv_t, h1_t, f32, nq, nkv, idqkv_t, rb.saved_inv(_F8_H1))
     else:
         dh1 = None
         dws = []
-        for off, n in zip(offs, widths):
-            dh1 = gemm_fp8(dqkv8[:, off:off + n], w_t[:, off:off + n], ib[_F8_DQKV], inv[_F8_WQKV], residual=dh1, out=dh1)
-            dws.append(gemm_fp8(dqkv_t[off:off + n], h1_t, ib[_F8_DQKV], inv[_F8_H1], out_f32=f32))
+        for off, n in zip((0, nq, nq + nkv), (nq, nkv, nkv)):
+            dh1 = rb.gemm(dqkv8[:, off:off + n], w_t[:, off:off + n], idqkv, iw_t, residual=dh1, out=dh1)
+            dws.append(rb.gemm(dqkv_t[off:off + n], h1_t, _seg(idqkv_t, off, n), rb.saved_inv(_F8_H1), out_f32=f32))
         dwq, dwk, dwv = dws
     dbq = dbk = dbv = None
     if ctx.has_bias:
@@ -985,7 +1305,7 @@ class DecoderLayerFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, ln1, wq, wk, wv, bq, bk, bv, wo, ln2, wg, wu, wd, wqb, wkb, wvb, wob, wgb, wub, wdb, cos, sin,
-                plan, H, KV, eps, hd=128, fp8=False):
+                plan, H, KV, eps, hd=128, fp8=False, fp8_recipe="tensorwise"):
         x2 = _rows2d(x)
         scale = 1.0 / math.sqrt(hd)
         if hd != 128 and (hd > 128 or hd % 8 or plan.tp is not None or plan.cp_group is not None):
@@ -1005,11 +1325,12 @@ class DecoderLayerFn(torch.autograd.Function):
             return _cp.cp_attn_fwd(q, k, v, plan, H, KV, scale)
 
         out, saved = block_forward(x2, ln1, wqb, wkb, wvb, bq, bk, bv, wob, ln2, wgb, wub, wdb, cos, sin, H, KV, eps, hd,
-                                   attend, tp, fp8=fp8)
+                                   attend, tp, fp8=fp8, fp8_recipe=fp8_recipe)
         ctx.save_for_backward(x2, ln1, ln2, wqb, wkb, wvb, wob, wgb, wub, wdb, cos, sin, *saved)
         ctx.plan, ctx.H, ctx.KV, ctx.scale, ctx.has_bias, ctx.hd, ctx.fp8 = plan, H, KV, scale, bq is not None, hd, fp8
         ctx.f32 = wq.dtype == torch.float32
         ctx.w_dtype = wq.dtype
+        ctx.fp8_recipe = fp8_recipe
         return out.view(x.shape)
 
     @staticmethod
@@ -1019,7 +1340,7 @@ class DecoderLayerFn(torch.autograd.Function):
             d2 = d2.to(BF16)
         if ctx.fp8:
             dx, *grads = _block_backward_fp8(ctx, ctx.saved_tensors, d2)
-            return (dx.view(dout.shape), *grads) + (None,) * 15
+            return (dx.view(dout.shape), *grads) + (None,) * 16
         (x2, ln1, ln2, wqb, wkb, wvb, wob, wgb, wub, wdb, cos, sin, rstd1, h1, q, k, v, o, lse, x1, rstd2, h2, g, u,
          hm) = ctx.saved_tensors
         H, KV, f32 = ctx.H, ctx.KV, ctx.f32
@@ -1087,11 +1408,15 @@ class DecoderLayerFn(torch.autograd.Function):
             tp.all_reduce_(dln1)
             tp.all_reduce_(dln2)
         return (dx.view(dout.shape), dln1.to(ln1.dtype), dwq, dwk, dwv, dbq, dbk, dbv, dwo, dln2.to(ln2.dtype), dwg, dwu,
-                dwd) + (None,) * 15
+                dwd) + (None,) * 16
 
 
-def decoder_layer(x, ln1, wq, wk, wv, bq, bk, bv, wo, ln2, wg, wu, wd, cos, sin, plan, H, KV, eps, hd=128, fp8=False):
-    """`fp8`: the seven projections in FP8 (the `float8_training` model config key; see block_forward)."""
+def decoder_layer(x, ln1, wq, wk, wv, bq, bk, bv, wo, ln2, wg, wu, wd, cos, sin, plan, H, KV, eps, hd=128, fp8=False, *,
+                  float8_recipe_name="tensorwise"):
+    """`fp8`: the seven projections in FP8 (the `float8_training` model config key; see block_forward), under
+    `float8_recipe_name` (the config key of that name: "tensorwise" or "rowwise")."""
+    if fp8:
+        check_fp8_recipe(float8_recipe_name)
     return DecoderLayerFn.apply(x, ln1, wq, wk, wv, bq, bk, bv, wo, ln2, wg, wu, wd, bf16_weight(wq), bf16_weight(wk),
                                 bf16_weight(wv), bf16_weight(wo), bf16_weight(wg), bf16_weight(wu), bf16_weight(wd),
-                                cos, sin, plan, H, KV, eps, hd, fp8)
+                                cos, sin, plan, H, KV, eps, hd, fp8, float8_recipe_name)
