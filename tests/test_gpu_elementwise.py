@@ -9,7 +9,7 @@ from touchnet_b200 import ops
 pytestmark = pytest.mark.gpu
 
 
-@pytest.mark.parametrize("rows,d", [(64, 4096), (200, 768), (33, 64), (1024, 2048)])
+@pytest.mark.parametrize("rows,d", [(64, 4096), (200, 768), (33, 64), (1024, 2048), (40, 8192), (7, 24)])
 @pytest.mark.parametrize("w_f32", [False, True])
 def test_rmsnorm_forward_backward(rows, d, w_f32):
     dev = require_cuda()

@@ -83,6 +83,13 @@ struct GemmParams {
   // indexed by the output column; EPI 1: [2N], the gate rows then the up rows)
   const float* inv_sa;
   const float* inv_sb;
+  // plain epilogue (EPI 0 / 2): output columns [n_store, N) - less than one 16-byte chunk, when the row length in bytes
+  // is not a multiple of 16 - are written with ordinary stores to d (row stride ldd), because the TMA store writes
+  // whole 16-byte chunks and would write past N into the caller's memory; the output map then ends at n_store.
+  // n_store = N: no such columns.
+  int n_store;
+  void* d;
+  int64_t ldd;
 };
 
 // Operand and output tensor maps.  d[]: EPI 0/2 the output (d_seg: one map per segment), EPI 1 H / G / U, EPI 3 dG / dU;
@@ -519,7 +526,26 @@ gemm_kernel(const __grid_constant__ GemmMaps tm, const GemmParams p) {
             *pd = v;
           }
         };
-        emit(false, fill, p.R != nullptr, add_residual, store1(dmap, x0, yd));
+        emit(false, fill, p.R != nullptr, add_residual, [=](uint8_t* buf) {
+          if (x0 < p.n_store) tma_store_2d(dmap, buf, x0, yd);   // the map ends at n_store: it clips the rest
+          tma_store_commit();
+        });
+      }
+      if (p.n_store < p.N && n0 + BN > p.n_store && t < 64 && y0 + t < p.M) {
+        // the ragged tail [n_store, N) of the last column tile (only tn_gemm_bf16 sets n_store < N, without segments):
+        // one 16-byte chunk of each row of the sub-tile staged last, read after the accumulator is dead; the next
+        // emit() synchronises the warpgroup before it writes that buffer again
+        const int xt = p.n_store - (p.n_store - n0) % SW;          // first column of that sub-tile
+        const uint8_t* sub = stg + (sbuf ^ 1) * SUB_BYTES;
+        const int q = (p.n_store - xt) / CW;
+        const uint4 v = *reinterpret_cast<const uint4*>(sub + t * 128 + ((q ^ (t & 7)) << 4));
+        const int64_t off = int64_t(y0 + t) * p.ldd + p.n_store;
+#pragma unroll
+        for (int e = 0; e < CW - 1; ++e)
+          if (p.n_store + e < p.N) {
+            if (EPI == 2) static_cast<float*>(p.d)[off + e] = reinterpret_cast<const float*>(&v)[e];
+            else static_cast<bf16*>(p.d)[off + e] = reinterpret_cast<const bf16*>(&v)[e];
+          }
       }
     }
   }
@@ -567,6 +593,7 @@ static GemmParams base_params(int M, int N, int K, int tile_n, int kb = BK) {
   p.num_m = (M + BM - 1) / BM;
   p.num_n = (N + tile_n - 1) / tile_n;
   p.num_k = (K + kb - 1) / kb;
+  p.n_store = N;
   p.group = gemm_group();
   // L2 policy: inside a raster group the `group` A strips are re-read by every wave, a B strip is consumed within
   // about one wave -> A evict-last, B evict-first (tn_set_gemm_l2_hints; default off)
@@ -646,11 +673,13 @@ extern "C" int tn_gemm_bf16(const void* A, int64_t lda, int a_mn, const void* B,
   const int bn = pick_bn(M, N, 1);
   GemmParams p = base_params(M, N, K, bn);
   p.R = R; p.ldr = ldr;
+  p.n_store = N & ~(d_f32 ? 3 : 7);   // whole 16-byte chunks go out by TMA, the rest by ordinary stores
+  p.d = D; p.ldd = ldd;
   GemmMaps tm;
   int rc;
   if ((rc = map_operand(&tm.a, A, a_mn, uint64_t(M), uint64_t(K), lda, BM))) return rc;
   if ((rc = map_operand(&tm.b[0], B, b_mn, uint64_t(N), uint64_t(K), ldb, bn))) return rc;
-  if ((rc = map_output(&tm.d[0], D, d_f32, uint64_t(M), uint64_t(N), ldd))) return rc;
+  if ((rc = map_output(&tm.d[0], D, d_f32, uint64_t(M), uint64_t(p.n_store > 0 ? p.n_store : N), ldd))) return rc;
   tm.b[1] = tm.b[2] = tm.b[0];
   tm.d[1] = tm.d[2] = tm.d[0];
 

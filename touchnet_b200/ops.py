@@ -37,6 +37,15 @@ def _rows2d(t: torch.Tensor) -> torch.Tensor:
     return t2
 
 
+def _dense_rows(t: torch.Tensor) -> torch.Tensor:
+    """2-D `t` with row stride equal to its width, for the kernels that address row r at r * cols (RMSNorm, the SwiGLU
+    backward, the embedding add).  Copies only when `t` is not already laid out so; `_rows2d` views with a wider row
+    stride (a column slice, a gradient coming back through torch.cat) are the case this exists for."""
+    if t.stride(-1) == 1 and (t.shape[0] <= 1 or t.stride(0) == t.shape[1]):
+        return t
+    return t.contiguous()
+
+
 # ---------------------------------------------------------------------------------------------------------------
 # bf16 working copies of fp32 master weights (what FSDP2's MixedPrecisionPolicy does at all-gather time,
 # ref: touchnet/models/helper_func.py:163; at 1 GPU the reference stays fp32, SURVEY 9.1 - we compute in bf16 always)
@@ -558,11 +567,16 @@ _F8_D2, _F8_DG, _F8_DU, _F8_DX1, _F8_DQKV = range(5)
 
 
 def swiglu_bwd(g, u, dh, dg_out=None, du_out=None):
+    """(dG, dU) of hm = silu(g)*u.  The kernel reads and writes all five [M, N] tensors with one row stride, N."""
     M, N = g.shape
-    dg = torch.empty_like(g) if dg_out is None else dg_out
-    du = torch.empty_like(u) if du_out is None else du_out
+    g, u, dh = _dense_rows(g), _dense_rows(u), _dense_rows(dh)
+    dg = torch.empty((M, N), dtype=BF16, device=g.device) if dg_out is None else dg_out
+    du = torch.empty((M, N), dtype=BF16, device=g.device) if du_out is None else du_out
+    for t, name in ((dg, "dg_out"), (du, "du_out")):
+        if t.shape != (M, N) or t.stride(-1) != 1 or (M > 1 and t.stride(0) != N):
+            raise _lib.TouchNetB200Error(f"swiglu_bwd: {name} must be [{M}, {N}] with row stride {N}")
     _lib.call("tn_swiglu_bwd_bf16", g.data_ptr(), u.data_ptr(), dh.data_ptr(), dg.data_ptr(), du.data_ptr(), M, N,
-              g.stride(0), _st())
+              N, _st())
     return dg, du
 
 
@@ -570,6 +584,9 @@ def rmsnorm_fwd(x: torch.Tensor, w: torch.Tensor, eps: float, residual: Optional
     """Returns (y, s, rstd): s = x (+ residual) is the tensor that was normalised."""
     _chk(x, "x", BF16)
     rows, d = x.shape
+    x = _dense_rows(x)
+    if residual is not None:
+        residual = _dense_rows(residual)
     y = torch.empty_like(x)
     rstd = torch.empty(rows, dtype=torch.float32, device=x.device)
     s = torch.empty_like(x) if residual is not None else x
@@ -590,6 +607,9 @@ def rmsnorm_bwd(s: torch.Tensor, dy: torch.Tensor, w: torch.Tensor, rstd: torch.
     if _norm_partials is None:
         _norm_partials = _lib.load().tn_rmsnorm_bwd_num_partials()
     rows, d = s.shape
+    s, dy = _dense_rows(s), _dense_rows(dy)
+    if ds_extra is not None:
+        ds_extra = _dense_rows(ds_extra)
     ds = torch.empty_like(s)
     part = torch.empty((_norm_partials, d), dtype=torch.float32, device=s.device)
     dw = torch.empty(d, dtype=torch.float32, device=s.device)
@@ -816,6 +836,8 @@ def embed_add(input_ids: Optional[torch.Tensor], embed: Optional[torch.Tensor], 
     dev = (proj if proj is not None else input_ids).device
     e = torch.empty((rows, d), dtype=BF16, device=dev)
     emb = None if embed is None else embed.detach()
+    if proj is not None:
+        proj = _dense_rows(proj)
     _lib.call("tn_embed_add_bf16", None if input_ids is None else input_ids.data_ptr(),
               None if emb is None else emb.data_ptr(), int(emb is not None and emb.dtype == torch.float32),
               None if proj is None else proj.data_ptr(), e.data_ptr(),
