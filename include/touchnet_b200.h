@@ -288,6 +288,25 @@ int tn_greedy_select_slots_bf16(const void* logits, int64_t ld, int n_rows, cons
                                 int32_t* finished, const int32_t* limit, float repetition_penalty,
                                 int no_repeat_ngram_size, int64_t eos, int64_t pad, tn_stream_t stream);
 
+/* Multinomial sampling over cache slots (generation.generate_many with do_sample=True).
+ *   tn_sample_select_slots: tn_greedy_select_slots with the argmax replaced by a draw from HF's sampling distribution:
+ *     the processed fp32 logits divided by temperature (> 0; 1 skips it), then top-k (0 or >= V skips it: every token
+ *     >= the k-th largest value is kept, ties included), then top-p in [0, 1] (1 skips it: a group of equal values v is
+ *     kept iff the kept mass of the values <= v is > (1 - top_p) times the kept total; the maximum always stays), then
+ *     softmax.  Token weights are exp(x - max) in 2^40 fixed point, so every sum is exact in any order; a token whose
+ *     weight rounds to 0 (total probability < V * 2^-40) is never drawn.  The draw is Philox4x32-10 with key = seed and
+ *     counter (length[slot], 0, stream key): a 64-bit r picks the target floor(r * Z / 2^64) in the kept total Z and the
+ *     token is the one whose interval of the prefix sums in index order holds it.  The stream key of a mapped row is
+ *     row_key[r] (HOST array beside row_slot), stored into stream_key[slot]; other rows read stream_key[slot] (device,
+ *     [B] int64).  A row with a NaN, an infinite maximum or every token banned takes tn_greedy_select's pick.
+ */
+int tn_sample_select_slots_bf16(const void* logits, int64_t ld, int n_rows, const int32_t* row_slot,
+                                const int64_t* row_key, int B, int V, int64_t* history, int64_t ld_hist, int32_t* length,
+                                int64_t* positions, int64_t* next_ids, int32_t* finished, const int32_t* limit,
+                                int64_t* stream_key, float repetition_penalty, int no_repeat_ngram_size,
+                                float temperature, int top_k, float top_p, int64_t seed, int64_t eos, int64_t pad,
+                                tn_stream_t stream);
+
 /* ---------------------------------------------------------------------------------------------------------------
  * Audio frontend.
  *   tn_fbank: touchnet/data/functions.py:117-134 audio_compute_fbank → ta:compliance/kaldi.py:514-645 (snip_edges,

@@ -66,6 +66,8 @@ _SIGNATURES = {
                               _vp],
     "tn_greedy_select_slots_bf16": [_vp, _i64, _i, _vp, _i, _i, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _f, _i, _i64, _i64,
                                     _vp],
+    "tn_sample_select_slots_bf16": [_vp, _i64, _i, _vp, _vp, _i, _i, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _f, _i,
+                                    _f, _i, _f, _i64, _i64, _i64, _vp],
     "tn_kv_scatter_bf16": [_vp, _i64, _vp, _i64, _i64, _vp, _vp, _i64, _i64, _vp, _i, _i, _i, _i, _vp],
     "tn_slot_admit": [_vp, _i, _vp, _vp, _vp, _i64, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _i, _vp],
     "tn_fbank_f32": [_vp, _i, _vp, _vp, _i, _i64, _i, _i, _i, _vp, _vp, _i, _f, _vp, _vp],

@@ -1,4 +1,5 @@
-// touchnet_b200 :: autoregressive decoding - split-KV decode attention, KV-cache append, greedy token selection.
+// touchnet_b200 :: autoregressive decoding - split-KV decode attention, KV-cache append, greedy and sampled token
+// selection.
 //
 // Replaces what transformers' `generate(use_cache=True, do_sample=False, num_beams=1)` runs per new token when the
 // reference evaluates a model (touchnet/models/touch_audio/inference_touch_audio.py:170-192): the attention of one new
@@ -13,7 +14,8 @@
 //
 // Continuous batching (generation.generate_many) adds slot-addressed forms: a K/V scatter of a packed multi-prompt
 // prefill into chosen cache slots, the admission of those slots' decoding state, and a selection that holds finished /
-// idle slots still and stops a slot at its token limit.
+// idle slots still and stops a slot at its token limit.  Its sampling form (generate_many with do_sample=True) draws
+// from HF's temperature / top-k / top-p distribution with a counter-based Philox stream per prompt.
 //
 // Speculative decoding (generation.generate with assistant_model) adds the multi-query form of the decode attention
 // (Tq new rows per sequence, causal within the block, each row bit-identical to the single-query kernel at its own
@@ -22,6 +24,8 @@
 #include "../../include/touchnet_b200.h"
 #include "attn_common.cuh"
 #include "host.h"
+
+#include <curand_philox4x32_x.h>
 
 namespace tn {
 
@@ -269,6 +273,50 @@ __device__ __forceinline__ bool argmax_better(float x, int i, float best, int bi
 
 enum SelectMode { SEL_PLAIN, SEL_SLOTS, SEL_VERIFY };
 
+// HF's processor front, shared by the greedy and the sampling selections: the repetition set and the no-repeat-ngram
+// ban of slot b's history as two bitmaps bits[0, words) / bits[words, 2 words).  The history is the slot's
+// length[b] ids followed (VERIFY) by draft[0 .. extra).  Returns the history length; ends on a barrier.
+template <bool VERIFY>
+__device__ __forceinline__ int processor_front(uint32_t* bits, uint32_t* rep, uint32_t* ban, int words, int V,
+                                               const int64_t* __restrict__ history, int64_t ld_hist,
+                                               const int32_t* __restrict__ length, int b,
+                                               const int64_t* __restrict__ draft, int extra, float penalty, int ngram) {
+  const int tid = threadIdx.x;
+  for (int i = tid; i < 2 * words; i += SEL_THREADS) bits[i] = 0u;
+  __syncthreads();
+  const int n0 = length[b];
+  const int len = n0 + extra;
+  const int64_t* h0 = history + int64_t(b) * ld_hist;
+  const auto h = [&](int i) { return VERIFY && i >= n0 ? draft[i - n0] : h0[i]; };
+  if (penalty != 1.0f) {
+    for (int i = tid; i < len; i += SEL_THREADS) {
+      const int64_t id = h(i);
+      if (id >= 0 && id < V) atomicOr(&rep[id >> 5], 1u << (id & 31));
+    }
+  }
+  if (ngram > 0 && len + 1 >= ngram) {
+    // ngram i = h[i .. i+n-1]; its last id is banned when its first n-1 ids equal the last n-1 ids of the sequence
+    for (int i = tid; i + ngram <= len; i += SEL_THREADS) {
+      bool match = true;
+      for (int j = 0; j < ngram - 1 && match; ++j) match = h(i + j) == h(len - ngram + 1 + j);
+      const int64_t id = h(i + ngram - 1);
+      if (match && id >= 0 && id < V) atomicOr(&ban[id >> 5], 1u << (id & 31));
+    }
+  }
+  __syncthreads();
+  return len;
+}
+
+// logit v of a row after the processor front: the fp32 value, the repetition penalty, -inf where banned (the loop of
+// greedy_select_row spells the same three steps out: written through this helper it compiles to other registers)
+__device__ __forceinline__ float processed_logit(const bf16* __restrict__ row, int v, const uint32_t* rep,
+                                                 const uint32_t* ban, bool use_pen, float penalty) {
+  float x = __bfloat162float(row[v]);
+  if (use_pen && (rep[v >> 5] >> (v & 31) & 1u)) x = x < 0.f ? x * penalty : x / penalty;
+  if (ban[v >> 5] >> (v & 31) & 1u) x = -INFINITY;
+  return x;
+}
+
 // The body of the three selection kernels.  Logits row r selects for slot b (r == b without a slot map).  SEL_PLAIN is
 // tn_greedy_select_bf16: every row advances, finished rows take pad.  SEL_SLOTS is tn_greedy_select_slots_bf16: a
 // finished (or idle) slot does not advance at all (pad in next_ids, nothing else written), and a slot also finishes
@@ -294,29 +342,9 @@ __device__ __forceinline__ void greedy_select_row(
   const int words = (V + 31) / 32;
   uint32_t* rep = bits;
   uint32_t* ban = bits + words;
-  for (int i = tid; i < 2 * words; i += SEL_THREADS) bits[i] = 0u;
-  __syncthreads();
-  const int n0 = length[b];
-  const int len = n0 + extra;
-  const int64_t* h0 = history + int64_t(b) * ld_hist;
-  const auto h = [&](int i) { return VERIFY && i >= n0 ? draft[i - n0] : h0[i]; };
+  const int len = processor_front<VERIFY>(bits, rep, ban, words, V, history, ld_hist, length, b, draft, extra, penalty,
+                                          ngram);
   const bool use_pen = penalty != 1.0f;
-  if (use_pen) {
-    for (int i = tid; i < len; i += SEL_THREADS) {
-      const int64_t id = h(i);
-      if (id >= 0 && id < V) atomicOr(&rep[id >> 5], 1u << (id & 31));
-    }
-  }
-  if (ngram > 0 && len + 1 >= ngram) {
-    // ngram i = h[i .. i+n-1]; its last id is banned when its first n-1 ids equal the last n-1 ids of the sequence
-    for (int i = tid; i + ngram <= len; i += SEL_THREADS) {
-      bool match = true;
-      for (int j = 0; j < ngram - 1 && match; ++j) match = h(i + j) == h(len - ngram + 1 + j);
-      const int64_t id = h(i + ngram - 1);
-      if (match && id >= 0 && id < V) atomicOr(&ban[id >> 5], 1u << (id & 31));
-    }
-  }
-  __syncthreads();
   const bf16* row = logits + int64_t(r) * ld;
   float best = -INFINITY;
   int bi = -1;
@@ -433,6 +461,259 @@ __global__ void __launch_bounds__(SEL_THREADS, 1) greedy_select_slots_kernel(
   const int r = blockIdx.x;
   greedy_select_row<SEL_SLOTS>(logits, ld, V, history, ld_hist, length, positions, next_ids, finished, limit, penalty, ngram,
                           eos, pad, r, map.use_map ? map.slot[r] : r);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// multinomial sampling over cache slots: HF's processors, temperature, top-k, top-p, a counter-based Philox draw
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int SMP_BINS = 2048;                   // radix digits of 11, 11 and 10 bits over the 32-bit order key
+constexpr float SMP_ONE = 1099511627776.f;       // 2^40: fixed-point weight of the row maximum
+
+struct SampleMap {
+  SlotMap slots;
+  int64_t key[SEL_MAX_MAP];                      // mapped rows: the prompt's stream key, stored into stream_key[slot]
+};
+
+// order-preserving uint32 key of a non-NaN float; -0 and +0 are one value, so they get one key
+__device__ __forceinline__ uint32_t order_key(float x) {
+  const uint32_t u = __float_as_uint(x == 0.f ? 0.f : x);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+
+// exp(x - m) in fixed point (2^40 at the maximum m); 0 below about m - 28.4, where the token is never drawn
+__device__ __forceinline__ unsigned long long fixed_weight(float x, float m) {
+  return __float2ull_rn(__expf(x - m) * SMP_ONE);
+}
+
+// Inclusive scan of one u64 per thread in thread order over the CTA; returns the exclusive prefix, *total the sum.
+// Every thread of the CTA calls it (it holds two barriers and reuses `scratch` [32]).
+__device__ __forceinline__ unsigned long long block_scan_u64(unsigned long long x, unsigned long long* scratch,
+                                                             unsigned long long* total) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  unsigned long long inc = x;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const unsigned long long y = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= o) inc += y;
+  }
+  if (lane == 31) scratch[warp] = inc;
+  __syncthreads();
+  if (warp == 0) {
+    unsigned long long w = scratch[lane], wi = w;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const unsigned long long y = __shfl_up_sync(0xffffffffu, wi, o);
+      if (lane >= o) wi += y;
+    }
+    scratch[lane] = wi - w;                      // exclusive prefix of each warp
+    if (lane == 31) scratch[32] = wi;
+  }
+  __syncthreads();
+  *total = scratch[32];
+  return scratch[warp] + inc - x;
+}
+
+struct BinPick {
+  int bin;
+  unsigned long long above, total;
+};
+
+// The radix step of both thresholds: walking hist[0, nb) from the top bin down, the bin where the running sum reaches
+// `need` (the sum of the bins above it < need <= that sum + its own).  need_of(total of the histogram) gives `need`.
+template <typename T, typename Need>
+__device__ BinPick find_bin(const T* hist, int nb, Need need_of, unsigned long long* scratch, BinPick* out) {
+  const int per = nb / SEL_THREADS, top = nb - 1 - per * int(threadIdx.x);   // this thread's bins, descending
+  unsigned long long s = 0;
+  for (int i = 0; i < per; ++i) s += hist[top - i];
+  unsigned long long total;
+  unsigned long long a = block_scan_u64(s, scratch, &total);
+  const unsigned long long need = need_of(total);
+  for (int i = 0; i < per; ++i) {
+    const unsigned long long h = hist[top - i];
+    if (a < need && a + h >= need) *out = BinPick{top - i, a, total};
+    a += h;
+  }
+  __syncthreads();
+  const BinPick p = *out;
+  __syncthreads();                               // `out` and `hist` may be rewritten after this
+  return p;
+}
+
+// One CTA per logits row; the slot rules, state writes and idle handling of greedy_select_slots_kernel.  Passes over the
+// row (re-read from L2): the max, fused with the first top-k histogram; two more top-k histograms; three top-p mass
+// histograms; the kept mass of each warp's index range; then one warp walks its range to the drawn token.
+__global__ void __launch_bounds__(SEL_THREADS, 1) sample_select_slots_kernel(
+    const bf16* __restrict__ logits, int64_t ld, int V, int64_t* __restrict__ history, int64_t ld_hist,
+    int32_t* __restrict__ length, int64_t* __restrict__ positions, int64_t* __restrict__ next_ids,
+    int32_t* __restrict__ finished, const int32_t* __restrict__ limit, int64_t* __restrict__ stream_key, float penalty,
+    int ngram, float temperature, int top_k, float top_p, uint64_t seed, int64_t eos, int64_t pad,
+    const SampleMap map) {
+  extern __shared__ uint32_t bits[];             // [2][words]: repetition set, banned set
+  __shared__ unsigned long long s_hist[SMP_BINS];
+  __shared__ unsigned long long s_scan[33];
+  __shared__ BinPick s_pick;
+  __shared__ float s_val[SEL_THREADS / 32];
+  __shared__ int s_idx[SEL_THREADS / 32];
+  __shared__ int s_tok;
+  const int r = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int b = map.slots.use_map ? map.slots.slot[r] : r;
+  if (finished[b]) {                             // uniform over the CTA: no barrier has been reached yet
+    if (tid == 0) next_ids[b] = pad;
+    return;
+  }
+  const int64_t key = map.slots.use_map ? map.key[r] : stream_key[b];
+  uint32_t* cnt = reinterpret_cast<uint32_t*>(s_hist);
+  for (int i = tid; i < SMP_BINS; i += SEL_THREADS) s_hist[i] = 0ull;
+  const int words = (V + 31) / 32;
+  uint32_t* rep = bits;
+  uint32_t* ban = bits + words;
+  const int len = processor_front<false>(bits, rep, ban, words, V, history, ld_hist, length, b, nullptr, 0, penalty,
+                                         ngram);
+  const bool use_pen = penalty != 1.0f, use_temp = temperature != 1.0f;
+  const bool use_k = top_k > 0 && top_k < V, use_p = top_p < 1.0f;
+  const bf16* row = logits + int64_t(r) * ld;
+  const auto value = [&](int v) {                // TemperatureLogitsWarper: a true division, as HF divides
+    const float x = processed_logit(row, v, rep, ban, use_pen, penalty);
+    return use_temp ? x / temperature : x;
+  };
+  const auto commit = [&](int64_t tok) {         // one thread: the writes of greedy_select_slots_kernel
+    if (map.slots.use_map) stream_key[b] = key;
+    if (len < ld_hist) history[int64_t(b) * ld_hist + len] = tok;
+    next_ids[b] = tok;
+    length[b] = len + 1;
+    positions[b] += 1;
+    if (tok == eos || len + 1 == limit[b]) finished[b] = 1;
+  };
+
+  // pass 1: the argmax in argmax_better's order (the pick of a degenerate row) and the first top-k count histogram
+  float best = -INFINITY;
+  int bi = -1;
+  for (int v = tid; v < V; v += SEL_THREADS) {
+    const float x = value(v);
+    if (argmax_better(x, v, best, bi)) { best = x; bi = v; }
+    if (use_k && x == x) atomicAdd(&cnt[order_key(x) >> 21], 1u);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float ov = __shfl_xor_sync(0xffffffffu, best, o);
+    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+    if (argmax_better(ov, oi, best, bi)) { best = ov; bi = oi; }
+  }
+  if (lane == 0) { s_val[warp] = best; s_idx[warp] = bi; }
+  __syncthreads();
+  best = s_val[0]; bi = s_idx[0];
+  for (int w = 1; w < SEL_THREADS / 32; ++w)
+    if (argmax_better(s_val[w], s_idx[w], best, bi)) { best = s_val[w]; bi = s_idx[w]; }
+  const float m = best;
+  // a NaN, an infinite maximum or nothing drawable (every token banned): the greedy kernel's pick
+  if (!(m > -INFINITY && m < INFINITY)) {
+    if (tid == 0) commit(bi);
+    return;
+  }
+
+  // radix digit l covers key bits [shift(l), shift(l) + width(l)); keys whose higher bits equal `pre` take part
+  const auto width = [](int l) { return l < 2 ? 11 : 10; };
+  const auto shift = [](int l) { return l < 2 ? 21 - 11 * l : 0; };
+  const auto in_prefix = [&](uint32_t k, int l, uint32_t pre) {
+    return (uint64_t(k) >> (shift(l) + width(l))) == pre;
+  };
+  const auto digit = [&](uint32_t k, int l) { return (k >> shift(l)) & ((1u << width(l)) - 1u); };
+
+  // top-k: the k-th largest key (ties included: every key >= it is kept)
+  uint32_t lo_key = 0u;
+  if (use_k) {
+    uint32_t pre = 0u;
+    unsigned long long need = unsigned(top_k);
+    for (int l = 0; l < 3; ++l) {
+      if (l > 0) {
+        for (int i = tid; i < SMP_BINS; i += SEL_THREADS) cnt[i] = 0u;
+        __syncthreads();
+        for (int v = tid; v < V; v += SEL_THREADS) {
+          const uint32_t k = order_key(value(v));
+          if (in_prefix(k, l, pre)) atomicAdd(&cnt[digit(k, l)], 1u);
+        }
+        __syncthreads();
+      }
+      const BinPick p = find_bin(cnt, 1 << width(l), [&](unsigned long long) { return need; }, s_scan, &s_pick);
+      need -= p.above;
+      pre = (pre << width(l)) | uint32_t(p.bin);
+    }
+    lo_key = pre;
+  }
+
+  // top-p over the top-k set: the lowest value group whose kept mass strictly above it is < top_p * Z (the row maximum
+  // always stays); the mass is in fixed point, so every sum below is exact in any order
+  uint32_t t_key = lo_key;
+  if (use_p) {
+    if (top_p <= 0.f) {
+      t_key = order_key(m);
+    } else {
+      uint32_t pre = 0u;
+      unsigned long long need = 0;
+      for (int l = 0; l < 3; ++l) {
+        for (int i = tid; i < SMP_BINS; i += SEL_THREADS) s_hist[i] = 0ull;
+        __syncthreads();
+        for (int v = tid; v < V; v += SEL_THREADS) {
+          const float x = value(v);
+          const uint32_t k = order_key(x);
+          if (k >= lo_key && in_prefix(k, l, pre)) {
+            const unsigned long long w = fixed_weight(x, m);
+            if (w) atomicAdd(&s_hist[digit(k, l)], w);
+          }
+        }
+        __syncthreads();
+        const auto need_of = [&](unsigned long long total) {
+          // level 0: ceil(top_p * Z); an integer mass is < top_p * Z iff it is < this
+          return l == 0 ? (unsigned long long)ceil(double(top_p) * double(total)) : need;
+        };
+        const BinPick p = find_bin(s_hist, 1 << width(l), need_of, s_scan, &s_pick);
+        need = need_of(p.total) - p.above;
+        pre = (pre << width(l)) | uint32_t(p.bin);
+      }
+      t_key = pre;
+    }
+  }
+
+  // the kept mass of each warp's index range [warp * chunk, warp * chunk + chunk), then the draw in index order
+  const int chunk = ((words + 31) / 32) * 32;
+  const int v0 = warp * chunk, v1 = min(V, v0 + chunk);
+  const auto kept_weight = [&](int v) -> unsigned long long {
+    if (v >= v1) return 0ull;
+    const float x = value(v);
+    return order_key(x) >= t_key ? fixed_weight(x, m) : 0ull;
+  };
+  unsigned long long s = 0;
+  for (int v = v0 + lane; v < v1; v += 32) s += kept_weight(v);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  unsigned long long total;
+  const unsigned long long before = block_scan_u64(lane == 0 ? s : 0ull, s_scan, &total);
+  // Philox4x32-10 keyed by the seed, counter (position in the row, 0, stream key): a target in [0, Z)
+  const uint4 rnd = curand_Philox4x32_10(make_uint4(uint32_t(len), 0u, uint32_t(uint64_t(key)),
+                                                    uint32_t(uint64_t(key) >> 32)),
+                                         make_uint2(uint32_t(seed), uint32_t(seed >> 32)));
+  const unsigned long long target = __umul64hi((uint64_t(rnd.y) << 32) | rnd.x, total);
+  const unsigned long long w_before = __shfl_sync(0xffffffffu, before, 0);
+  if (target >= w_before && target < w_before + s) {   // this warp's range holds the target (uniform over the warp)
+    unsigned long long base = w_before;
+    for (int j = v0; j < v1; j += 32) {
+      const unsigned long long w = kept_weight(j + lane);
+      unsigned long long inc = w;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const unsigned long long y = __shfl_up_sync(0xffffffffu, inc, o);
+        if (lane >= o) inc += y;
+      }
+      const bool hit = target >= base + inc - w && target < base + inc;
+      if (__any_sync(0xffffffffu, hit)) {
+        if (hit) s_tok = j + lane;
+        break;
+      }
+      base += __shfl_sync(0xffffffffu, inc, 31);
+    }
+  }
+  __syncthreads();
+  if (tid == 0) commit(s_tok);
 }
 
 // grid (longest document, documents): row t of document j -> cache row t of slot j, 16-byte copies
@@ -603,33 +884,61 @@ extern "C" int tn_greedy_select_bf16(const void* logits, int64_t ld, int B, int 
       ld, V, history, ld_hist, length, positions, next_ids, finished, repetition_penalty, no_repeat_ngram_size, eos, pad);
 }
 
+// the checks of both slot selections; the host row -> slot map is checked and copied into `map` (passed by value)
+static int slot_select_args(const char* fn, const void* logits, int64_t ld, int n_rows, const int32_t* row_slot, int B,
+                            int V, const void* history, int64_t ld_hist, const void* length, const void* positions,
+                            const void* next_ids, const void* finished, const void* limit, SlotMap* map) {
+  TN_REQUIRE(logits && history && length && positions && next_ids && finished && limit, "%s: null pointer", fn);
+  TN_REQUIRE(n_rows > 0 && B > 0 && V > 0 && ld >= V && ld_hist > 0, "%s: bad dims n_rows=%d B=%d V=%d", fn, n_rows, B,
+             V);
+  TN_REQUIRE(row_slot || n_rows == B, "%s: bad dims: without a row -> slot map n_rows (%d) must equal B (%d)", fn,
+             n_rows, B);
+  TN_REQUIRE(!row_slot || n_rows <= SEL_MAX_MAP, "%s: at most %d mapped rows, got %d", fn, SEL_MAX_MAP, n_rows);
+  map->use_map = row_slot != nullptr;
+  for (int r = 0; row_slot && r < n_rows; ++r) {   // the map is host memory: checked here, passed by value
+    TN_REQUIRE(row_slot[r] >= 0 && row_slot[r] < B, "%s: slot %d out of range [0, %d)", fn, row_slot[r], B);
+    for (int q = 0; q < r; ++q) TN_REQUIRE(row_slot[q] != row_slot[r], "%s: slot %d named twice", fn, row_slot[r]);
+    map->slot[r] = row_slot[r];
+  }
+  return TN_OK;
+}
+
 extern "C" int tn_greedy_select_slots_bf16(const void* logits, int64_t ld, int n_rows, const int32_t* row_slot, int B,
                                            int V, int64_t* history, int64_t ld_hist, int32_t* length, int64_t* positions,
                                            int64_t* next_ids, int32_t* finished, const int32_t* limit,
                                            float repetition_penalty, int no_repeat_ngram_size, int64_t eos, int64_t pad,
                                            tn_stream_t stream_) {
   clear_error();
-  TN_REQUIRE(logits && history && length && positions && next_ids && finished && limit,
-             "tn_greedy_select_slots_bf16: null pointer");
-  TN_REQUIRE(n_rows > 0 && B > 0 && V > 0 && ld >= V && ld_hist > 0, "tn_greedy_select_slots_bf16: bad dims n_rows=%d "
-             "B=%d V=%d", n_rows, B, V);
-  TN_REQUIRE(row_slot || n_rows == B, "tn_greedy_select_slots_bf16: bad dims: without a row -> slot map n_rows (%d) "
-             "must equal B (%d)", n_rows, B);
-  TN_REQUIRE(!row_slot || n_rows <= SEL_MAX_MAP, "tn_greedy_select_slots_bf16: at most %d mapped rows, got %d",
-             SEL_MAX_MAP, n_rows);
   SlotMap map{};
-  map.use_map = row_slot != nullptr;
-  for (int r = 0; row_slot && r < n_rows; ++r) {   // the map is host memory: checked here, passed by value
-    TN_REQUIRE(row_slot[r] >= 0 && row_slot[r] < B, "tn_greedy_select_slots_bf16: slot %d out of range [0, %d)",
-               row_slot[r], B);
-    for (int q = 0; q < r; ++q)
-      TN_REQUIRE(row_slot[q] != row_slot[r], "tn_greedy_select_slots_bf16: slot %d named twice", row_slot[r]);
-    map.slot[r] = row_slot[r];
-  }
+  if (const int rc = slot_select_args("tn_greedy_select_slots_bf16", logits, ld, n_rows, row_slot, B, V, history, ld_hist,
+                                      length, positions, next_ids, finished, limit, &map)) return rc;
   return select_launch<greedy_select_slots_kernel>(
       "tn_greedy_select_slots_bf16", n_rows, V, repetition_penalty, no_repeat_ngram_size, stream_,
       static_cast<const bf16*>(logits), ld, V, history, ld_hist, length, positions, next_ids, finished, limit,
       repetition_penalty, no_repeat_ngram_size, eos, pad, map);
+}
+
+extern "C" int tn_sample_select_slots_bf16(const void* logits, int64_t ld, int n_rows, const int32_t* row_slot,
+                                           const int64_t* row_key, int B, int V, int64_t* history, int64_t ld_hist,
+                                           int32_t* length, int64_t* positions, int64_t* next_ids, int32_t* finished,
+                                           const int32_t* limit, int64_t* stream_key, float repetition_penalty,
+                                           int no_repeat_ngram_size, float temperature, int top_k, float top_p,
+                                           int64_t seed, int64_t eos, int64_t pad, tn_stream_t stream_) {
+  clear_error();
+  const char* fn = "tn_sample_select_slots_bf16";
+  SampleMap map{};
+  if (const int rc = slot_select_args(fn, logits, ld, n_rows, row_slot, B, V, history, ld_hist, length, positions,
+                                      next_ids, finished, limit, &map.slots)) return rc;
+  TN_REQUIRE(stream_key && (row_key || !row_slot), "%s: null pointer (stream_key, or row_key with a row -> slot map)",
+             fn);
+  TN_REQUIRE(temperature > 0.f && temperature < INFINITY, "%s: temperature must be a finite number > 0", fn);
+  TN_REQUIRE(top_k >= 0, "%s: top_k must be >= 0", fn);
+  TN_REQUIRE(top_p >= 0.f && top_p <= 1.f, "%s: top_p must be in [0, 1]", fn);
+  for (int r = 0; row_slot && r < n_rows; ++r) map.key[r] = row_key[r];
+  return select_launch<sample_select_slots_kernel>(
+      fn, n_rows, V, repetition_penalty, no_repeat_ngram_size, stream_, static_cast<const bf16*>(logits), ld, V, history,
+      ld_hist, length, positions, next_ids, finished, limit, stream_key, repetition_penalty, no_repeat_ngram_size,
+      temperature, top_k, top_p, uint64_t(seed), eos, pad, map);
 }
 
 extern "C" int tn_verify_select_bf16(const void* logits, int64_t ld, int B, int k, int V, const int64_t* draft,

@@ -15,7 +15,8 @@ repetition_penalty, no_repeat_ngram_size, max_new_tokens, ...)` on left-padded p
   generate_many
            continuous batching over many prompts: a cache of B slots, finished rows refilled with the next prompts
            (packed prefill into chosen slots: tn_kv_scatter_bf16, tn_slot_admit) while the captured decode step keeps
-           replaying (tn_greedy_select_slots_bf16 holds finished and idle slots still).
+           replaying (tn_greedy_select_slots_bf16 holds finished and idle slots still); do_sample=True draws the
+           tokens instead (tn_sample_select_slots_bf16: temperature, top-k, top-p, a Philox stream per prompt).
   speculative
            generate(assistant_model=draft): per round the draft proposes k tokens, the model scores them in one step of
            B*(k+1) rows (tn_attn_decode_multi_bf16) and keeps the longest prefix equal to its own picks plus its next
@@ -620,13 +621,35 @@ def _admit(model, cache: B200KVCache, limit: torch.Tensor, w: _Weights, batch, p
     select(_logits_last(w, x.index_select(0, last)), [slot for slot, _ in batch])
 
 
+def _sampling_args(temperature, top_k, top_p):
+    """HF's multinomial-sampling knobs, None -> transformers' defaults (temperature 1.0, top_k 50, top_p 1.0)."""
+    temperature = 1.0 if temperature is None else temperature
+    top_k = 50 if top_k is None else top_k
+    top_p = 1.0 if top_p is None else top_p
+    if (isinstance(temperature, bool) or not isinstance(temperature, (int, float))
+            or not 0.0 < float(temperature) < math.inf):
+        raise TouchNetB200Error(f"generate_many: temperature must be a finite number > 0, got {temperature}")
+    if isinstance(top_k, bool) or not isinstance(top_k, int) or top_k < 0:
+        raise TouchNetB200Error(f"generate_many: top_k must be an int >= 0, got {top_k}")
+    if isinstance(top_p, bool) or not isinstance(top_p, (int, float)) or not 0.0 <= float(top_p) <= 1.0:
+        raise TouchNetB200Error(f"generate_many: top_p must be in [0, 1], got {top_p}")
+    return float(temperature), min(int(top_k), 2**31 - 1), float(top_p)
+
+
 def generate_many(model, prompts, *, batch_size, max_new_tokens, eos_token_id, pad_token_id, repetition_penalty=1.0,
-                  no_repeat_ngram_size=0, max_prompt_length=None, cuda_graph: bool = True, stats: Optional[dict] = None):
-    """Greedy decoding of many prompts with continuous batching: a cache of `batch_size` slots; when a slot's row
-    finishes (eos or its token budget), its generated ids are copied out and the next prompt is prefilled into that slot
-    while the other slots keep decoding.  Per prompt, the result is what `generate` returns for that prompt alone
-    (HF greedy with the same processors), as a 1-D int64 tensor of the generated ids (eos included if reached, no
-    padding); the list is in input order.
+                  no_repeat_ngram_size=0, max_prompt_length=None, cuda_graph: bool = True, stats: Optional[dict] = None,
+                  do_sample: bool = False, temperature=None, top_k=None, top_p=None):
+    """Greedy decoding, or multinomial sampling, of many prompts with continuous batching: a cache of `batch_size`
+    slots; when a slot's row finishes (eos or its token budget), its generated ids are copied out and the next prompt is
+    prefilled into that slot while the other slots keep decoding.  Per prompt, the greedy result is what `generate`
+    returns for that prompt alone (HF greedy with the same processors), as a 1-D int64 tensor of the generated ids (eos
+    included if reached, no padding); the list is in input order.
+
+    do_sample=True draws each token from HF's sampling distribution (processors, then temperature, top_k, top_p; None
+    takes HF's defaults 1.0, 50, 1.0) with tn_sample_select_slots_bf16.  One 64-bit seed is taken from torch's default
+    CPU generator, so torch.manual_seed reproduces a call; prompt i draws from its own Philox stream (seed, i) at its
+    token positions, so its ids do not depend on batch_size, its slot, its neighbours or when it was admitted.  With
+    do_sample=False the three knobs are ignored, as HF ignores them in greedy search.
 
     prompts          iterable of dicts: input_ids [T], optional input_features [T, F] (TouchAudio), attention_mask [T]
                      (doc ids or 0/1, last document rule of `generate`), position_ids [T]
@@ -647,6 +670,8 @@ def generate_many(model, prompts, *, batch_size, max_new_tokens, eos_token_id, p
     else:
         max_budget = int(max_new_tokens)
     _validate(max_budget, eos_token_id, pad_token_id, repetition_penalty, no_repeat_ngram_size, False, 1, {})
+    if do_sample:
+        temperature, top_k, top_p = _sampling_args(temperature, top_k, top_p)
     _check_scope(model)
     B = int(batch_size)
     if B < 1:
@@ -676,15 +701,24 @@ def generate_many(model, prompts, *, batch_size, max_new_tokens, eos_token_id, p
         w = _Weights(lm)
         cache = B200KVCache(model, B, max_len + max_budget, device=dev)
         limit = torch.zeros(B, dtype=torch.int32, device=dev)
+        stream_key = torch.zeros(B, dtype=torch.int64, device=dev)    # the index of the prompt in each slot
+        seed = int(torch.randint(-2**63, 2**63 - 1, (), dtype=torch.int64)) if do_sample else 0
         cache.finished.fill_(1)               # every slot starts idle
         nan_flag = None if audio is None else audio._nan_flag
         admission_events = []
         admissions = 0
 
         def select(logits, slots=None):
-            ops.greedy_select_slots(logits, cache.history, cache.kv_end, cache.positions, cache.next_ids,
-                                    cache.finished, limit, float(repetition_penalty), int(no_repeat_ngram_size), eos,
-                                    pad, row_slot=slots)
+            if do_sample:
+                ops.sample_select_slots(logits, cache.history, cache.kv_end, cache.positions, cache.next_ids,
+                                        cache.finished, limit, stream_key, float(repetition_penalty),
+                                        int(no_repeat_ngram_size), temperature, top_k, top_p, seed, eos, pad,
+                                        row_slot=slots,
+                                        row_key=None if slots is None else [slot_prompt[s].index for s in slots])
+            else:
+                ops.greedy_select_slots(logits, cache.history, cache.kv_end, cache.positions, cache.next_ids,
+                                        cache.finished, limit, float(repetition_penalty), int(no_repeat_ngram_size),
+                                        eos, pad, row_slot=slots)
 
         def admit(free) -> None:
             nonlocal count, admissions
@@ -701,6 +735,8 @@ def generate_many(model, prompts, *, batch_size, max_new_tokens, eos_token_id, p
                 count += 1
             for i in range(0, len(batch), _ADMIT_MAX):
                 chunk = batch[i:i + _ADMIT_MAX]
+                for slot, p in chunk:             # before the admission: its selection reads the prompts' indices
+                    slot_prompt[slot] = p
                 ev = None
                 if stats is not None and dev.type == "cuda":
                     ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
@@ -710,8 +746,6 @@ def generate_many(model, prompts, *, batch_size, max_new_tokens, eos_token_id, p
                 if ev is not None:
                     ev[1].record()
                     admission_events.append(ev)
-                for slot, p in chunk:
-                    slot_prompt[slot] = p
 
         step = _captured(lambda: select(decode_step(model, cache, weights=w)), cuda_graph and dev.type == "cuda")
         admit(list(range(B)))

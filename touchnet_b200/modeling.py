@@ -428,7 +428,7 @@ class B200LlamaForCausalLM(nn.Module):
         return generation.generate(self, input_ids, None, attention_mask, position_ids, **kwargs)
 
     def generate_many(self, prompts, **kwargs: Any):
-        """Greedy decoding of many prompts with continuous batching (see generation.generate_many)."""
+        """Greedy decoding or sampling of many prompts with continuous batching (see generation.generate_many)."""
         from . import generation
         return generation.generate_many(self, prompts, **kwargs)
 

@@ -830,6 +830,25 @@ def greedy_select_slots(logits, history, length, positions, next_ids, finished, 
               int(no_repeat_ngram_size), int(eos), int(pad), _st())
 
 
+def sample_select_slots(logits, history, length, positions, next_ids, finished, limit, stream_key,
+                        repetition_penalty: float, no_repeat_ngram_size: int, temperature: float, top_k: int,
+                        top_p: float, seed: int, eos: int, pad: int, row_slot=None, row_key=None):
+    """greedy_select_slots with the argmax replaced by a multinomial draw (temperature, top-k, top-p; see
+    tn_sample_select_slots_bf16).  stream_key [B] int64 holds each slot's stream key; a mapped row r (row_slot given)
+    draws with row_key[r] and stores it into stream_key[row_slot[r]].  The draw of a slot is a function of (seed, its
+    stream key, its length, its processed logits) only."""
+    n, V = _select_dims(logits, history, length, positions, next_ids, finished)
+    _chk(limit, "limit", torch.int32); _chk(stream_key, "stream_key", torch.int64)
+    tab = None if row_slot is None else _host_i32(row_slot)
+    keys = None if row_key is None else torch.tensor(row_key, dtype=torch.int64).reshape(-1).contiguous()
+    _lib.call("tn_sample_select_slots_bf16", logits.data_ptr(), logits.stride(0), n,
+              None if tab is None else tab.data_ptr(), None if keys is None else keys.data_ptr(), history.shape[0], V,
+              history.data_ptr(), history.stride(0), length.data_ptr(), positions.data_ptr(), next_ids.data_ptr(),
+              finished.data_ptr(), limit.data_ptr(), stream_key.data_ptr(), float(repetition_penalty),
+              int(no_repeat_ngram_size), float(temperature), int(top_k), float(top_p), int(seed), int(eos), int(pad),
+              _st())
+
+
 def embed_add(input_ids: Optional[torch.Tensor], embed: Optional[torch.Tensor], proj: Optional[torch.Tensor],
               rows: int, d: int, nan_flag: Optional[torch.Tensor] = None):
     """E = embed[input_ids] + proj (either may be None)."""
