@@ -307,6 +307,30 @@ int tn_sample_select_slots_bf16(const void* logits, int64_t ld, int n_rows, cons
                                 float temperature, int top_k, float top_p, int64_t seed, int64_t eos, int64_t pad,
                                 tn_stream_t stream);
 
+/* Speculative sampling (generation.generate_many with assistant_model and do_sample=True; Leviathan et al. 2023,
+ * Algorithm 1) over B slots and k draft tokens per slot.
+ *   tn_spec_sample_verify: logits [B*(k+1), V] of the model (row b*(k+1) + j) and draft_logits [B*k, V] of the draft
+ *     (row b*k + j, the logits the draft drew draft[b, j] from), draft [B, k] int64 (device).  For a slot with
+ *     finished == 0, p_j and q_j are tn_sample_select_slots's distributions (same processors, temperature, top_k,
+ *     top_p and 2^40 fixed-point weights) of target row j and draft row j over history[b, 0:length[b]] followed by
+ *     draft[b, 0:j].  Position j < k accepts draft[b, j] = x iff floor(r * wq(x) * Zp / 2^64) < wp(x) * Zq in exact
+ *     integers, r the 64-bit Philox4x32-10 draw (key seed, counter (length[b] + j, 1, stream_key[b])): probability
+ *     min(1, p_j(x) / q_j(x)) within 2^-64.  At the first rejection n (or n = k) the row emits one token drawn from
+ *     max(0, wp * Zq - wq * Zp) (p_k itself at n = k) in index order with the draw of counter (length[b] + n, 2,
+ *     stream_key[b]).  A target row with a NaN, an infinite maximum or every token banned emits its greedy pick and
+ *     stops there; a degenerate draft row's q is a point mass on its greedy pick.  The emitted tokens (accepted
+ *     drafts, then the last) are committed as tn_verify_select commits its picks: cut after the first eos and when
+ *     length reaches limit[b].  A finished slot does not advance (next_ids = pad, nothing else written).
+ *     picks [B, k+1] int64 (device scratch) receives, for each slot not finished, x at an accepted position and ~t at
+ *     the position that emitted t (later positions are computed but never read).
+ */
+int tn_spec_sample_verify_bf16(const void* logits, int64_t ld, const void* draft_logits, int64_t ldd, int B, int k,
+                               int V, const int64_t* draft, int64_t* history, int64_t ld_hist, int32_t* length,
+                               int64_t* positions, int64_t* next_ids, int32_t* finished, const int32_t* limit,
+                               const int64_t* stream_key, int64_t* picks, float repetition_penalty,
+                               int no_repeat_ngram_size, float temperature, int top_k, float top_p, int64_t seed,
+                               int64_t eos, int64_t pad, tn_stream_t stream);
+
 /* ---------------------------------------------------------------------------------------------------------------
  * Audio frontend.
  *   tn_fbank: touchnet/data/functions.py:117-134 audio_compute_fbank → ta:compliance/kaldi.py:514-645 (snip_edges,

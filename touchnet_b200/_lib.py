@@ -68,6 +68,8 @@ _SIGNATURES = {
                                     _vp],
     "tn_sample_select_slots_bf16": [_vp, _i64, _i, _vp, _vp, _i, _i, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _f, _i,
                                     _f, _i, _f, _i64, _i64, _i64, _vp],
+    "tn_spec_sample_verify_bf16": [_vp, _i64, _vp, _i64, _i, _i, _i, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                   _f, _i, _f, _i, _f, _i64, _i64, _i64, _vp],
     "tn_kv_scatter_bf16": [_vp, _i64, _vp, _i64, _i64, _vp, _vp, _i64, _i64, _vp, _i, _i, _i, _i, _vp],
     "tn_slot_admit": [_vp, _i, _vp, _vp, _vp, _i64, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _i, _vp],
     "tn_fbank_f32": [_vp, _i, _vp, _vp, _i, _i64, _i, _i, _i, _vp, _vp, _i, _f, _vp, _vp],
@@ -130,7 +132,7 @@ def load(path: str | None = None) -> ctypes.CDLL:
 
 # kernels launched per entry point (for bench.py's `gpu_launches` claim)
 _LAUNCHES = {"tn_attn_prep": 3, "tn_attn_bwd_bf16": 3, "tn_attn_decode_bf16": 2, "tn_attn_decode_multi_bf16": 2,
-             "tn_verify_select_bf16": 2, "tn_logmel_power_f32": 2,
+             "tn_verify_select_bf16": 2, "tn_spec_sample_verify_bf16": 2, "tn_logmel_power_f32": 2,
              "tn_rmsnorm_bwd_bf16": 2, "tn_pack_layout_i64": 2}
 launch_count = 0
 _hooks = []   # callables(name, phase) with phase in {"pre", "post"}; bench.py uses them to time kernel classes

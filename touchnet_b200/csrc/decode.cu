@@ -404,15 +404,16 @@ __global__ void __launch_bounds__(SEL_THREADS) verify_pick_kernel(
                                 ngram, 0, 0, r, b, draft + int64_t(b) * k, j, picks + r);
 }
 
-// one thread per row: emit picks 0..n (n = the leading draft tokens equal to their pick), stopping after an eos and at
-// the row's limit, then advance the row's state as the slot selection does for one token
-__global__ void verify_commit_kernel(const int64_t* __restrict__ picks, const int64_t* __restrict__ draft, int k, int B,
-                                     int64_t* __restrict__ history, int64_t ld_hist, int32_t* __restrict__ length,
-                                     int64_t* __restrict__ positions, int64_t* __restrict__ next_ids,
-                                     int32_t* __restrict__ finished, const int32_t* __restrict__ limit, int64_t eos,
-                                     int64_t pad) {
-  const int b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b >= B) return;
+// The commit of both verify selections, one thread per row: emit picks 0..n, stopping after an eos and at the row's
+// limit, then advance the row's state as the slot selection does for one token.  Greedy (verify_pick_kernel's picks):
+// n = the leading draft tokens equal to their pick.  SAMPLED (spec_sample_verify_kernel's picks): a pick x >= 0 is an
+// accepted draft token, ~t the row's last token t.  A finished row does not advance.
+template <bool SAMPLED>
+__device__ __forceinline__ void commit_row(const int64_t* __restrict__ picks, const int64_t* __restrict__ draft, int k,
+                                           int b, int64_t* __restrict__ history, int64_t ld_hist,
+                                           int32_t* __restrict__ length, int64_t* __restrict__ positions,
+                                           int64_t* __restrict__ next_ids, int32_t* __restrict__ finished,
+                                           const int32_t* __restrict__ limit, int64_t eos, int64_t pad) {
   if (finished[b]) {   // a finished row does not advance
     next_ids[b] = pad;
     return;
@@ -424,15 +425,34 @@ __global__ void verify_commit_kernel(const int64_t* __restrict__ picks, const in
   int64_t tok;
   bool stop;
   do {
-    tok = pk[c];
+    tok = SAMPLED && pk[c] < 0 ? ~pk[c] : pk[c];
     if (len + c < ld_hist) history[int64_t(b) * ld_hist + len + c] = tok;
     ++c;
-    stop = tok == eos || len + c >= lim || c == k + 1 || d[c - 1] != tok;
+    stop = tok == eos || len + c >= lim || c == k + 1 || (SAMPLED ? pk[c - 1] < 0 : d[c - 1] != tok);
   } while (!stop);
   length[b] = len + c;
   positions[b] += c;
   next_ids[b] = tok;
   if (tok == eos || len + c >= lim) finished[b] = 1;
+}
+
+__global__ void verify_commit_kernel(const int64_t* __restrict__ picks, const int64_t* __restrict__ draft, int k, int B,
+                                     int64_t* __restrict__ history, int64_t ld_hist, int32_t* __restrict__ length,
+                                     int64_t* __restrict__ positions, int64_t* __restrict__ next_ids,
+                                     int32_t* __restrict__ finished, const int32_t* __restrict__ limit, int64_t eos,
+                                     int64_t pad) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  commit_row<false>(picks, draft, k, b, history, ld_hist, length, positions, next_ids, finished, limit, eos, pad);
+}
+
+__global__ void spec_commit_kernel(const int64_t* __restrict__ picks, int k, int B, int64_t* __restrict__ history,
+                                   int64_t ld_hist, int32_t* __restrict__ length, int64_t* __restrict__ positions,
+                                   int64_t* __restrict__ next_ids, int32_t* __restrict__ finished,
+                                   const int32_t* __restrict__ limit, int64_t eos, int64_t pad) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  commit_row<true>(picks, picks, k, b, history, ld_hist, length, positions, next_ids, finished, limit, eos, pad);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -485,24 +505,46 @@ __device__ __forceinline__ unsigned long long fixed_weight(float x, float m) {
   return __float2ull_rn(__expf(x - m) * SMP_ONE);
 }
 
-// Inclusive scan of one u64 per thread in thread order over the CTA; returns the exclusive prefix, *total the sum.
-// Every thread of the CTA calls it (it holds two barriers and reuses `scratch` [32]).
-__device__ __forceinline__ unsigned long long block_scan_u64(unsigned long long x, unsigned long long* scratch,
-                                                             unsigned long long* total) {
+// Exact integer weights: u64 for one distribution's weights (<= 2^40 each, V * 2^40 < 2^64 in total), u128 for the
+// speculative residual (products of a weight and a total, < 2^100 each).  Warp shuffles of both.
+typedef unsigned __int128 u128;
+__device__ __forceinline__ unsigned long long shfl_up(unsigned long long x, int o) {
+  return __shfl_up_sync(0xffffffffu, x, o);
+}
+__device__ __forceinline__ unsigned long long shfl_xor(unsigned long long x, int o) {
+  return __shfl_xor_sync(0xffffffffu, x, o);
+}
+__device__ __forceinline__ unsigned long long shfl_idx(unsigned long long x, int l) {
+  return __shfl_sync(0xffffffffu, x, l);
+}
+__device__ __forceinline__ u128 shfl_up(u128 x, int o) {
+  return (u128(shfl_up((unsigned long long)(x >> 64), o)) << 64) | shfl_up((unsigned long long)x, o);
+}
+__device__ __forceinline__ u128 shfl_xor(u128 x, int o) {
+  return (u128(shfl_xor((unsigned long long)(x >> 64), o)) << 64) | shfl_xor((unsigned long long)x, o);
+}
+__device__ __forceinline__ u128 shfl_idx(u128 x, int l) {
+  return (u128(shfl_idx((unsigned long long)(x >> 64), l)) << 64) | shfl_idx((unsigned long long)x, l);
+}
+
+// Inclusive scan of one W per thread in thread order over the CTA; returns the exclusive prefix, *total the sum.
+// Every thread of the CTA calls it (it holds two barriers and reuses `scratch` [33]).
+template <typename W>
+__device__ __forceinline__ W block_scan(W x, W* scratch, W* total) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  unsigned long long inc = x;
+  W inc = x;
 #pragma unroll
   for (int o = 1; o < 32; o <<= 1) {
-    const unsigned long long y = __shfl_up_sync(0xffffffffu, inc, o);
+    const W y = shfl_up(inc, o);
     if (lane >= o) inc += y;
   }
   if (lane == 31) scratch[warp] = inc;
   __syncthreads();
   if (warp == 0) {
-    unsigned long long w = scratch[lane], wi = w;
+    W w = scratch[lane], wi = w;
 #pragma unroll
     for (int o = 1; o < 32; o <<= 1) {
-      const unsigned long long y = __shfl_up_sync(0xffffffffu, wi, o);
+      const W y = shfl_up(wi, o);
       if (lane >= o) wi += y;
     }
     scratch[lane] = wi - w;                      // exclusive prefix of each warp
@@ -526,7 +568,7 @@ __device__ BinPick find_bin(const T* hist, int nb, Need need_of, unsigned long l
   unsigned long long s = 0;
   for (int i = 0; i < per; ++i) s += hist[top - i];
   unsigned long long total;
-  unsigned long long a = block_scan_u64(s, scratch, &total);
+  unsigned long long a = block_scan(s, scratch, &total);
   const unsigned long long need = need_of(total);
   for (int i = 0; i < per; ++i) {
     const unsigned long long h = hist[top - i];
@@ -539,52 +581,31 @@ __device__ BinPick find_bin(const T* hist, int nb, Need need_of, unsigned long l
   return p;
 }
 
-// One CTA per logits row; the slot rules, state writes and idle handling of greedy_select_slots_kernel.  Passes over the
-// row (re-read from L2): the max, fused with the first top-k histogram; two more top-k histograms; three top-p mass
-// histograms; the kept mass of each warp's index range; then one warp walks its range to the drawn token.
-__global__ void __launch_bounds__(SEL_THREADS, 1) sample_select_slots_kernel(
-    const bf16* __restrict__ logits, int64_t ld, int V, int64_t* __restrict__ history, int64_t ld_hist,
-    int32_t* __restrict__ length, int64_t* __restrict__ positions, int64_t* __restrict__ next_ids,
-    int32_t* __restrict__ finished, const int32_t* __restrict__ limit, int64_t* __restrict__ stream_key, float penalty,
-    int ngram, float temperature, int top_k, float top_p, uint64_t seed, int64_t eos, int64_t pad,
-    const SampleMap map) {
-  extern __shared__ uint32_t bits[];             // [2][words]: repetition set, banned set
-  __shared__ unsigned long long s_hist[SMP_BINS];
-  __shared__ unsigned long long s_scan[33];
-  __shared__ BinPick s_pick;
-  __shared__ float s_val[SEL_THREADS / 32];
-  __shared__ int s_idx[SEL_THREADS / 32];
-  __shared__ int s_tok;
-  const int r = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int b = map.slots.use_map ? map.slots.slot[r] : r;
-  if (finished[b]) {                             // uniform over the CTA: no barrier has been reached yet
-    if (tid == 0) next_ids[b] = pad;
-    return;
-  }
-  const int64_t key = map.slots.use_map ? map.key[r] : stream_key[b];
-  uint32_t* cnt = reinterpret_cast<uint32_t*>(s_hist);
-  for (int i = tid; i < SMP_BINS; i += SEL_THREADS) s_hist[i] = 0ull;
-  const int words = (V + 31) / 32;
-  uint32_t* rep = bits;
-  uint32_t* ban = bits + words;
-  const int len = processor_front<false>(bits, rep, ban, words, V, history, ld_hist, length, b, nullptr, 0, penalty,
-                                         ngram);
-  const bool use_pen = penalty != 1.0f, use_temp = temperature != 1.0f;
-  const bool use_k = top_k > 0 && top_k < V, use_p = top_p < 1.0f;
-  const bf16* row = logits + int64_t(r) * ld;
-  const auto value = [&](int v) {                // TemperatureLogitsWarper: a true division, as HF divides
-    const float x = processed_logit(row, v, rep, ban, use_pen, penalty);
-    return use_temp ? x / temperature : x;
-  };
-  const auto commit = [&](int64_t tok) {         // one thread: the writes of greedy_select_slots_kernel
-    if (map.slots.use_map) stream_key[b] = key;
-    if (len < ld_hist) history[int64_t(b) * ld_hist + len] = tok;
-    next_ids[b] = tok;
-    length[b] = len + 1;
-    positions[b] += 1;
-    if (tok == eos || len + 1 == limit[b]) finished[b] = 1;
-  };
+// Shared memory of the sampling passes (declared by each kernel, used by the passes below)
+struct SampleShared {
+  unsigned long long* hist;                      // [SMP_BINS]; its first half is also the u32 count histogram
+  unsigned long long* scan;                      // [33]
+  BinPick* pick;
+  float* val;                                    // [SEL_THREADS / 32]
+  int* idx;                                      // [SEL_THREADS / 32]
+};
 
+// What the passes find in one processed row: its maximum m at bi (argmax_better's order, the pick of a degenerate row)
+// and the order key t_key of the kept set's lowest value (a token is kept iff order_key(value) >= t_key).  A row whose
+// m is not finite (a NaN, an infinite maximum, every token banned) is degenerate and has no t_key.
+struct SampleCut {
+  float m;
+  int bi;
+  uint32_t t_key;
+};
+
+// The passes over value(v), v in [0, V) (re-read from L2): the max, fused with the first top-k histogram; two more
+// top-k histograms; three top-p mass histograms.  sh.hist must be zero, and a barrier reached, before the call.
+template <typename Value>
+__device__ __forceinline__ SampleCut sample_cut(Value value, int V, int top_k, float top_p, const SampleShared& sh) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const bool use_k = top_k > 0 && top_k < V, use_p = top_p < 1.0f;
+  uint32_t* cnt = reinterpret_cast<uint32_t*>(sh.hist);
   // pass 1: the argmax in argmax_better's order (the pick of a degenerate row) and the first top-k count histogram
   float best = -INFINITY;
   int bi = -1;
@@ -599,17 +620,13 @@ __global__ void __launch_bounds__(SEL_THREADS, 1) sample_select_slots_kernel(
     const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
     if (argmax_better(ov, oi, best, bi)) { best = ov; bi = oi; }
   }
-  if (lane == 0) { s_val[warp] = best; s_idx[warp] = bi; }
+  if (lane == 0) { sh.val[warp] = best; sh.idx[warp] = bi; }
   __syncthreads();
-  best = s_val[0]; bi = s_idx[0];
+  best = sh.val[0]; bi = sh.idx[0];
   for (int w = 1; w < SEL_THREADS / 32; ++w)
-    if (argmax_better(s_val[w], s_idx[w], best, bi)) { best = s_val[w]; bi = s_idx[w]; }
+    if (argmax_better(sh.val[w], sh.idx[w], best, bi)) { best = sh.val[w]; bi = sh.idx[w]; }
   const float m = best;
-  // a NaN, an infinite maximum or nothing drawable (every token banned): the greedy kernel's pick
-  if (!(m > -INFINITY && m < INFINITY)) {
-    if (tid == 0) commit(bi);
-    return;
-  }
+  if (!(m > -INFINITY && m < INFINITY)) return SampleCut{m, bi, 0u};
 
   // radix digit l covers key bits [shift(l), shift(l) + width(l)); keys whose higher bits equal `pre` take part
   const auto width = [](int l) { return l < 2 ? 11 : 10; };
@@ -634,7 +651,7 @@ __global__ void __launch_bounds__(SEL_THREADS, 1) sample_select_slots_kernel(
         }
         __syncthreads();
       }
-      const BinPick p = find_bin(cnt, 1 << width(l), [&](unsigned long long) { return need; }, s_scan, &s_pick);
+      const BinPick p = find_bin(cnt, 1 << width(l), [&](unsigned long long) { return need; }, sh.scan, sh.pick);
       need -= p.above;
       pre = (pre << width(l)) | uint32_t(p.bin);
     }
@@ -651,14 +668,14 @@ __global__ void __launch_bounds__(SEL_THREADS, 1) sample_select_slots_kernel(
       uint32_t pre = 0u;
       unsigned long long need = 0;
       for (int l = 0; l < 3; ++l) {
-        for (int i = tid; i < SMP_BINS; i += SEL_THREADS) s_hist[i] = 0ull;
+        for (int i = tid; i < SMP_BINS; i += SEL_THREADS) sh.hist[i] = 0ull;
         __syncthreads();
         for (int v = tid; v < V; v += SEL_THREADS) {
           const float x = value(v);
           const uint32_t k = order_key(x);
           if (k >= lo_key && in_prefix(k, l, pre)) {
             const unsigned long long w = fixed_weight(x, m);
-            if (w) atomicAdd(&s_hist[digit(k, l)], w);
+            if (w) atomicAdd(&sh.hist[digit(k, l)], w);
           }
         }
         __syncthreads();
@@ -666,54 +683,240 @@ __global__ void __launch_bounds__(SEL_THREADS, 1) sample_select_slots_kernel(
           // level 0: ceil(top_p * Z); an integer mass is < top_p * Z iff it is < this
           return l == 0 ? (unsigned long long)ceil(double(top_p) * double(total)) : need;
         };
-        const BinPick p = find_bin(s_hist, 1 << width(l), need_of, s_scan, &s_pick);
+        const BinPick p = find_bin(sh.hist, 1 << width(l), need_of, sh.scan, sh.pick);
         need = need_of(p.total) - p.above;
         pre = (pre << width(l)) | uint32_t(p.bin);
       }
       t_key = pre;
     }
   }
+  return SampleCut{m, bi, t_key};
+}
 
-  // the kept mass of each warp's index range [warp * chunk, warp * chunk + chunk), then the draw in index order
+// the fixed-point weight of token v in the distribution `c` of value(): exp(x - m) * 2^40 if kept, else 0
+template <typename Value>
+__device__ __forceinline__ unsigned long long kept_weight(Value value, int v, const SampleCut& c) {
+  const float x = value(v);
+  return order_key(x) >= c.t_key ? fixed_weight(x, c.m) : 0ull;
+}
+
+// Inverse-CDF draw in index order over the integer weights weight(v) of v in [0, V): each warp sums its index range
+// [warp * chunk, warp * chunk + chunk), a block scan gives the total Z, target_of(Z) in [0, Z) picks the token whose
+// interval of the prefix sums holds it, and the warp whose range holds the target walks it.  The token is in *s_tok
+// after the closing barrier (not written when Z = 0).
+template <typename W, typename Weight, typename Target>
+__device__ __forceinline__ void draw_index_order(Weight weight, int V, Target target_of, W* scan, int* s_tok) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int words = (V + 31) / 32;
   const int chunk = ((words + 31) / 32) * 32;
   const int v0 = warp * chunk, v1 = min(V, v0 + chunk);
-  const auto kept_weight = [&](int v) -> unsigned long long {
-    if (v >= v1) return 0ull;
-    const float x = value(v);
-    return order_key(x) >= t_key ? fixed_weight(x, m) : 0ull;
-  };
-  unsigned long long s = 0;
-  for (int v = v0 + lane; v < v1; v += 32) s += kept_weight(v);
+  const auto range_weight = [&](int v) -> W { return v >= v1 ? W(0) : weight(v); };
+  W s = 0;
+  for (int v = v0 + lane; v < v1; v += 32) s += range_weight(v);
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-  unsigned long long total;
-  const unsigned long long before = block_scan_u64(lane == 0 ? s : 0ull, s_scan, &total);
-  // Philox4x32-10 keyed by the seed, counter (position in the row, 0, stream key): a target in [0, Z)
-  const uint4 rnd = curand_Philox4x32_10(make_uint4(uint32_t(len), 0u, uint32_t(uint64_t(key)),
-                                                    uint32_t(uint64_t(key) >> 32)),
-                                         make_uint2(uint32_t(seed), uint32_t(seed >> 32)));
-  const unsigned long long target = __umul64hi((uint64_t(rnd.y) << 32) | rnd.x, total);
-  const unsigned long long w_before = __shfl_sync(0xffffffffu, before, 0);
-  if (target >= w_before && target < w_before + s) {   // this warp's range holds the target (uniform over the warp)
-    unsigned long long base = w_before;
+  for (int o = 16; o > 0; o >>= 1) s += shfl_xor(s, o);
+  W total;
+  const W before = block_scan(lane == 0 ? s : W(0), scan, &total);
+  const W target = target_of(total);
+  const W w_before = shfl_idx(before, 0);
+  if (target >= w_before && target - w_before < s) {   // this warp's range holds the target (uniform over the warp)
+    W rest = target - w_before;                        // the target's offset past the chunks walked so far
     for (int j = v0; j < v1; j += 32) {
-      const unsigned long long w = kept_weight(j + lane);
-      unsigned long long inc = w;
+      const W w = range_weight(j + lane);
+      W inc = w;
 #pragma unroll
       for (int o = 1; o < 32; o <<= 1) {
-        const unsigned long long y = __shfl_up_sync(0xffffffffu, inc, o);
+        const W y = shfl_up(inc, o);
         if (lane >= o) inc += y;
       }
-      const bool hit = target >= base + inc - w && target < base + inc;
+      const bool hit = rest >= inc - w && rest < inc;
       if (__any_sync(0xffffffffu, hit)) {
-        if (hit) s_tok = j + lane;
+        if (hit) *s_tok = j + lane;
         break;
       }
-      base += __shfl_sync(0xffffffffu, inc, 31);
+      rest -= shfl_idx(inc, 31);
     }
   }
   __syncthreads();
+}
+
+// Philox4x32-10 keyed by the seed at counter (position in the row, purpose, stream key): 64 random bits
+constexpr uint32_t RND_TOKEN = 0, RND_ACCEPT = 1, RND_RESIDUAL = 2;   // purposes
+__device__ __forceinline__ uint64_t philox_u64(uint64_t seed, int pos, uint32_t purpose, int64_t key) {
+  const uint4 rnd = curand_Philox4x32_10(make_uint4(uint32_t(pos), purpose, uint32_t(uint64_t(key)),
+                                                    uint32_t(uint64_t(key) >> 32)),
+                                         make_uint2(uint32_t(seed), uint32_t(seed >> 32)));
+  return (uint64_t(rnd.y) << 32) | rnd.x;
+}
+
+// One CTA per logits row; the slot rules, state writes and idle handling of greedy_select_slots_kernel.  Passes over the
+// row (re-read from L2): those of sample_cut; the kept mass of each warp's index range; then one warp walks its range to
+// the drawn token.
+__global__ void __launch_bounds__(SEL_THREADS, 1) sample_select_slots_kernel(
+    const bf16* __restrict__ logits, int64_t ld, int V, int64_t* __restrict__ history, int64_t ld_hist,
+    int32_t* __restrict__ length, int64_t* __restrict__ positions, int64_t* __restrict__ next_ids,
+    int32_t* __restrict__ finished, const int32_t* __restrict__ limit, int64_t* __restrict__ stream_key, float penalty,
+    int ngram, float temperature, int top_k, float top_p, uint64_t seed, int64_t eos, int64_t pad,
+    const SampleMap map) {
+  extern __shared__ uint32_t bits[];             // [2][words]: repetition set, banned set
+  __shared__ unsigned long long s_hist[SMP_BINS];
+  __shared__ unsigned long long s_scan[33];
+  __shared__ BinPick s_pick;
+  __shared__ float s_val[SEL_THREADS / 32];
+  __shared__ int s_idx[SEL_THREADS / 32];
+  __shared__ int s_tok;
+  const int r = blockIdx.x, tid = threadIdx.x;
+  const int b = map.slots.use_map ? map.slots.slot[r] : r;
+  if (finished[b]) {                             // uniform over the CTA: no barrier has been reached yet
+    if (tid == 0) next_ids[b] = pad;
+    return;
+  }
+  const int64_t key = map.slots.use_map ? map.key[r] : stream_key[b];
+  for (int i = tid; i < SMP_BINS; i += SEL_THREADS) s_hist[i] = 0ull;
+  const int words = (V + 31) / 32;
+  uint32_t* rep = bits;
+  uint32_t* ban = bits + words;
+  const int len = processor_front<false>(bits, rep, ban, words, V, history, ld_hist, length, b, nullptr, 0, penalty,
+                                         ngram);
+  const bool use_pen = penalty != 1.0f, use_temp = temperature != 1.0f;
+  const bf16* row = logits + int64_t(r) * ld;
+  const auto value = [&](int v) {                // TemperatureLogitsWarper: a true division, as HF divides
+    const float x = processed_logit(row, v, rep, ban, use_pen, penalty);
+    return use_temp ? x / temperature : x;
+  };
+  const auto commit = [&](int64_t tok) {         // one thread: the writes of greedy_select_slots_kernel
+    if (map.slots.use_map) stream_key[b] = key;
+    if (len < ld_hist) history[int64_t(b) * ld_hist + len] = tok;
+    next_ids[b] = tok;
+    length[b] = len + 1;
+    positions[b] += 1;
+    if (tok == eos || len + 1 == limit[b]) finished[b] = 1;
+  };
+  const SampleCut c = sample_cut(value, V, top_k, top_p, SampleShared{s_hist, s_scan, &s_pick, s_val, s_idx});
+  // a NaN, an infinite maximum or nothing drawable (every token banned): the greedy kernel's pick
+  if (!(c.m > -INFINITY && c.m < INFINITY)) {
+    if (tid == 0) commit(c.bi);
+    return;
+  }
+  // the draw in index order: a target in [0, Z)
+  draw_index_order<unsigned long long>(
+      [&](int v) { return kept_weight(value, v, c); }, V,
+      [&](unsigned long long total) { return __umul64hi(philox_u64(seed, len, RND_TOKEN, key), total); }, s_scan,
+      &s_tok);
   if (tid == 0) commit(s_tok);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// speculative sampling (Leviathan et al. 2023, Algorithm 1): grid (k + 1, B), then the commit of verify_select
+// ---------------------------------------------------------------------------------------------------------------
+// floor(r * X / 2^64), exact for X < 2^114 (the 64 x 64 high half carries the low word's share)
+__device__ __forceinline__ u128 mul_hi64(uint64_t r, u128 X) {
+  return u128(r) * uint64_t(X >> 64) + __umul64hi(r, uint64_t(X));
+}
+
+// CTA (j, b): position j of slot b's block, whose context is the slot's history followed by draft[b, 0 .. j).  p is the
+// sampling distribution of target row b*(k+1) + j, q that of draft row b*k + j (j < k), both with the same processor
+// bitmaps and passes as sample_select_slots_kernel, in 2^40 fixed point: p(v) = wp(v) / Zp, q(v) = wq(v) / Zq.  A
+// degenerate draft row drew its greedy pick: q is a point mass there (wq = 1 at that pick, Zq = 1).
+//   j < k: accept x = draft[b, j] iff floor(r * wq(x) * Zp / 2^64) < wp(x) * Zq for the 64-bit Philox draw r of
+//          (len, RND_ACCEPT): probability min(1, p(x) / q(x)) to within 2^-64.  Accepted: picks[b, j] = x.
+//   otherwise (rejected, or j = k): the token drawn from max(0, wp * Zq - wq * Zp) (wq = 0, Zq = 1 at j = k: p itself)
+//          in index order with the draw (len, RND_RESIDUAL); picks[b, j] = ~token.
+// A degenerate target row stops the row there with its greedy pick: picks[b, j] = ~pick.  Finished slots: nothing.
+__global__ void __launch_bounds__(SEL_THREADS, 1) spec_sample_verify_kernel(
+    const bf16* __restrict__ logits, int64_t ld, const bf16* __restrict__ dlogits, int64_t ldd, int V,
+    const int64_t* __restrict__ draft, int k, const int64_t* __restrict__ history, int64_t ld_hist,
+    const int32_t* __restrict__ length, const int32_t* __restrict__ finished, const int64_t* __restrict__ stream_key,
+    int64_t* __restrict__ picks, float penalty, int ngram, float temperature, int top_k, float top_p, uint64_t seed) {
+  extern __shared__ uint32_t bits[];             // [2][words]: repetition set, banned set
+  __shared__ unsigned long long s_hist[SMP_BINS];
+  __shared__ u128 s_scan[33];
+  __shared__ BinPick s_pick;
+  __shared__ float s_val[SEL_THREADS / 32];
+  __shared__ int s_idx[SEL_THREADS / 32];
+  __shared__ int s_tok;
+  __shared__ SampleCut s_cut[2];                 // p, q
+  __shared__ unsigned long long s_tot[2];        // Zp, Zq
+  __shared__ bool s_point;                       // q is a point mass (a degenerate draft row)
+  const int j = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
+  if (finished[b]) return;                       // uniform over the CTA
+  unsigned long long* scan64 = reinterpret_cast<unsigned long long*>(s_scan);
+  const SampleShared sh{s_hist, scan64, &s_pick, s_val, s_idx};
+  for (int i = tid; i < SMP_BINS; i += SEL_THREADS) s_hist[i] = 0ull;
+  const int words = (V + 31) / 32;
+  uint32_t* rep = bits;
+  uint32_t* ban = bits + words;
+  const int64_t* d = draft + int64_t(b) * k;
+  const int len = processor_front<true>(bits, rep, ban, words, V, history, ld_hist, length, b, d, j, penalty, ngram);
+  const bool use_pen = penalty != 1.0f, use_temp = temperature != 1.0f;
+  const bf16* prow = logits + (int64_t(b) * (k + 1) + j) * ld;
+  const bf16* qrow = dlogits + (int64_t(b) * k + min(j, k - 1)) * ldd;
+  const auto value_p = [&](int v) {
+    const float x = processed_logit(prow, v, rep, ban, use_pen, penalty);
+    return use_temp ? x / temperature : x;
+  };
+  const auto value_q = [&](int v) {
+    const float x = processed_logit(qrow, v, rep, ban, use_pen, penalty);
+    return use_temp ? x / temperature : x;
+  };
+  const auto total = [&](auto weight) {          // sum of weight(v) over the row (ends on a barrier)
+    unsigned long long s = 0, z;
+    for (int v = tid; v < V; v += SEL_THREADS) s += weight(v);
+    block_scan(s, scan64, &z);
+    __syncthreads();
+    return z;
+  };
+  int64_t* out = picks + int64_t(b) * (k + 1) + j;
+  {
+    const SampleCut P = sample_cut(value_p, V, top_k, top_p, sh);
+    if (!(P.m > -INFINITY && P.m < INFINITY)) {
+      if (tid == 0) *out = ~int64_t(P.bi);
+      return;
+    }
+    const unsigned long long Zp = total([&](int v) { return kept_weight(value_p, v, P); });
+    if (tid == 0) { s_cut[0] = P; s_tot[0] = Zp; }
+  }
+  if (j < k) {
+    for (int i = tid; i < SMP_BINS; i += SEL_THREADS) s_hist[i] = 0ull;
+    __syncthreads();
+    const SampleCut Q = sample_cut(value_q, V, top_k, top_p, sh);
+    const bool q_point = !(Q.m > -INFINITY && Q.m < INFINITY);
+    const unsigned long long Zq = q_point ? 1ull : total([&](int v) { return kept_weight(value_q, v, Q); });
+    if (tid == 0) { s_cut[1] = Q; s_tot[1] = Zq; s_point = q_point; }
+  }
+  __syncthreads();
+  // p's and q's cuts and totals come back from shared memory: nothing of the p pass stays live in registers across
+  // the q pass (a 1024-thread CTA has 64 registers per thread)
+  const SampleCut P = s_cut[0];
+  const unsigned long long Zp = s_tot[0];
+  const SampleCut Q = j < k ? s_cut[1] : SampleCut{0.f, -1, 0u};
+  const unsigned long long Zq = j < k ? s_tot[1] : 1ull;
+  const bool q_point = j < k && s_point;
+  const auto wp = [&](int v) { return kept_weight(value_p, v, P); };
+  const auto wq = [&](int v) -> unsigned long long {
+    if (j == k) return 0ull;
+    if (q_point) return v == Q.bi ? 1ull : 0ull;
+    return kept_weight(value_q, v, Q);
+  };
+  const int64_t key = stream_key[b];
+  if (j < k) {
+    const int64_t x = d[j];
+    const bool drawable = x >= 0 && x < V;
+    const u128 A = drawable ? u128(wp(int(x))) * Zq : u128(0);
+    const u128 Bq = drawable ? u128(wq(int(x))) * Zp : u128(0);
+    if (mul_hi64(philox_u64(seed, len, RND_ACCEPT, key), Bq) < A) {   // uniform over the CTA
+      if (tid == 0) *out = x;
+      return;
+    }
+  }
+  if (tid == 0) s_tok = P.bi;                    // an empty residual (x not drawable from q, and q == p): p's argmax
+  const auto residual = [&](int v) -> u128 {
+    const u128 a = u128(wp(v)) * Zq, c = u128(wq(v)) * Zp;
+    return a > c ? a - c : u128(0);
+  };
+  draw_index_order<u128>(residual, V, [&](u128 R) { return mul_hi64(philox_u64(seed, len, RND_RESIDUAL, key), R); },
+                         s_scan, &s_tok);
+  if (tid == 0) *out = ~int64_t(s_tok);
 }
 
 // grid (longest document, documents): row t of document j -> cache row t of slot j, 16-byte copies
@@ -959,6 +1162,33 @@ extern "C" int tn_verify_select_bf16(const void* logits, int64_t ld, int B, int 
   if (rc != TN_OK) return rc;
   verify_commit_kernel<<<(B + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream_)>>>(
       picks, draft, k, B, history, ld_hist, length, positions, next_ids, finished, limit, eos, pad);
+  TN_CHECK_CUDA(cudaGetLastError());
+  return TN_OK;
+}
+
+extern "C" int tn_spec_sample_verify_bf16(const void* logits, int64_t ld, const void* draft_logits, int64_t ldd, int B,
+                                          int k, int V, const int64_t* draft, int64_t* history, int64_t ld_hist,
+                                          int32_t* length, int64_t* positions, int64_t* next_ids, int32_t* finished,
+                                          const int32_t* limit, const int64_t* stream_key, int64_t* picks,
+                                          float repetition_penalty, int no_repeat_ngram_size, float temperature,
+                                          int top_k, float top_p, int64_t seed, int64_t eos, int64_t pad,
+                                          tn_stream_t stream_) {
+  clear_error();
+  const char* fn = "tn_spec_sample_verify_bf16";
+  TN_REQUIRE(logits && draft_logits && draft && history && length && positions && next_ids && finished && limit &&
+                 stream_key && picks, "%s: null pointer", fn);
+  TN_REQUIRE(B > 0 && k > 0 && V > 0 && ld >= V && ldd >= V && ld_hist > 0, "%s: bad dims B=%d k=%d V=%d", fn, B, k, V);
+  TN_REQUIRE(B <= 65535 && k < 65535, "%s: grid too large (B=%d, k=%d)", fn, B, k);
+  TN_REQUIRE(temperature > 0.f && temperature < INFINITY, "%s: temperature must be a finite number > 0", fn);
+  TN_REQUIRE(top_k >= 0, "%s: top_k must be >= 0", fn);
+  TN_REQUIRE(top_p >= 0.f && top_p <= 1.f, "%s: top_p must be in [0, 1]", fn);
+  const int rc = select_launch<spec_sample_verify_kernel>(
+      fn, dim3(k + 1, B), V, repetition_penalty, no_repeat_ngram_size, stream_, static_cast<const bf16*>(logits), ld,
+      static_cast<const bf16*>(draft_logits), ldd, V, draft, k, history, ld_hist, length, finished, stream_key, picks,
+      repetition_penalty, no_repeat_ngram_size, temperature, top_k, top_p, uint64_t(seed));
+  if (rc != TN_OK) return rc;
+  spec_commit_kernel<<<(B + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream_)>>>(
+      picks, k, B, history, ld_hist, length, positions, next_ids, finished, limit, eos, pad);
   TN_CHECK_CUDA(cudaGetLastError());
   return TN_OK;
 }

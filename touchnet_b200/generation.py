@@ -442,6 +442,51 @@ def _multi_ws(cache: B200KVCache, Tq: int, s_attn: int) -> torch.Tensor:
     return torch.empty(int(n), dtype=torch.float32, device=cache.data.device)
 
 
+class _SpecRound:
+    """One round of speculative decoding over the model's cache tc and the draft's cache dc (both [B, S_gen + k] rows),
+    device state only, so that it is captured once as a CUDA graph: bring the draft's state to the model's (and
+    `copies`, further (dst, src) pairs), a two-token draft step (the last two accepted tokens: the draft never fed its
+    last proposal when all were accepted), k - 1 one-token draft steps, each followed by draft_select(logits, j) and its
+    token copied from dc.next_ids into drafts[:, j], then the verify step of B*(k+1) rows and verify(logits).
+
+    The verify step attends to the first S_gen rows of tc only, the cache length of decoding without a draft, so that
+    every row sums in that decode step's split order; a query row clipped there lies past its slot's limit, so its pick
+    is never emitted.  A slot with no tokens (idle in generate_many) reads history row 0; its draft steps append nothing
+    and attend to nothing, its verify step appends rows [0, k) of its own slot and attends to them; every read and write
+    stays inside the slot, and its selections hold it still."""
+
+    def __init__(self, model, draft, tc, dc, w, wd, k, S_gen, draft_select, verify, copies=()):
+        dev = tc.data.device
+        self.model, self.draft, self.tc, self.dc, self.w, self.wd = model, draft, tc, dc, w, wd
+        self.k, self.S_gen = k, S_gen
+        self.draft_select, self.verify = draft_select, verify
+        self.copies = ((dc.history, tc.history), (dc.kv_end, tc.kv_end), (dc.positions, tc.positions),
+                       (dc.finished, tc.finished)) + tuple(copies)
+        self.drafts = torch.zeros((tc.B, k), dtype=torch.int64, device=dev)
+        self.end = torch.zeros(tc.B, dtype=torch.int32, device=dev)
+        self.ar = torch.arange(k + 1, dtype=torch.int64, device=dev)
+        self.ws, self.dws = _multi_ws(tc, k + 1, S_gen), _multi_ws(dc, 2, dc.S_cap)
+
+    def __call__(self):
+        tc, dc, wd, k, ar, B = self.tc, self.dc, self.wd, self.k, self.ar, self.tc.B
+        for dst, src in self.copies:
+            dst.copy_(src)
+        # the last two accepted tokens, at positions - 1 and positions
+        ids2 = dc.history.gather(1, (dc.kv_end.to(torch.int64)[:, None] - 2 + ar[None, :2]).clamp_(min=0))
+        x = _block_step(self.draft, dc, wd, ids2, dc.positions[:, None] - 1 + ar[None, :2], dc.kv_end, self.dws,
+                        dc.S_cap)
+        self.draft_select(_logits_last(wd, x.view(B, 2, -1)[:, 1].contiguous()), 0)
+        self.drafts[:, 0].copy_(dc.next_ids)
+        for j in range(1, k):
+            self.draft_select(decode_step(self.draft, dc, weights=wd), j)
+            self.drafts[:, j].copy_(dc.next_ids)
+        # verify: next_ids and the k proposals at positions + 0..k, appended at rows [kv_end - 1, kv_end + k)
+        torch.add(tc.kv_end, k, out=self.end)
+        x = _block_step(self.model, tc, self.w, torch.cat([tc.next_ids[:, None], self.drafts], 1),
+                        tc.positions[:, None] + ar, self.end, self.ws, self.S_gen)
+        self.verify(_logits_last(self.w, x))
+
+
 def generate_speculative(model, input_ids, input_features=None, attention_mask=None, position_ids=None, *,
                          assistant_model, max_new_tokens, eos_token_id, pad_token_id, num_assistant_tokens=None,
                          num_assistant_tokens_schedule=None, repetition_penalty=1.0, no_repeat_ngram_size=0,
@@ -482,11 +527,7 @@ def generate_speculative(model, input_ids, input_features=None, attention_mask=N
         dc = B200KVCache(draft, B, S_cap, device=dev)
         flags = (None if audio is None else audio._nan_flag, None if daudio is None else daudio._nan_flag)
         limit = torch.full((B,), T + max_new, dtype=torch.int32, device=dev)
-        drafts = torch.zeros((B, k), dtype=torch.int64, device=dev)
         picks = torch.zeros((B, k + 1), dtype=torch.int64, device=dev)
-        end = torch.zeros(B, dtype=torch.int32, device=dev)
-        ar = torch.arange(k + 1, dtype=torch.int64, device=dev)
-        ws, dws = _multi_ws(tc, k + 1, S_gen), _multi_ws(dc, 2, S_cap)
 
         ops.greedy_select(prefill(model, tc, input_ids, input_features, attention_mask, position_ids, weights=w),
                           tc.history, tc.kv_end, tc.positions, tc.next_ids, tc.finished, penalty, ngram, eos, pad)
@@ -495,26 +536,14 @@ def generate_speculative(model, input_ids, input_features=None, attention_mask=N
         def draft_select(logits, j):
             ops.greedy_select(logits, dc.history, dc.kv_end, dc.positions, dc.next_ids, dc.finished, penalty, ngram,
                               eos, pad)
-            drafts[:, j].copy_(dc.next_ids)
 
-        def round_():
-            for dst, src in ((dc.history, tc.history), (dc.kv_end, tc.kv_end), (dc.positions, tc.positions),
-                             (dc.finished, tc.finished)):
-                dst.copy_(src)
-            # the last two accepted tokens, at positions - 1 and positions
-            ids2 = dc.history.gather(1, dc.kv_end.to(torch.int64)[:, None] - 2 + ar[None, :2])
-            x = _block_step(draft, dc, wd, ids2, dc.positions[:, None] - 1 + ar[None, :2], dc.kv_end, dws, S_cap)
-            draft_select(_logits_last(wd, x.view(B, 2, -1)[:, 1].contiguous()), 0)
-            for j in range(1, k):
-                draft_select(decode_step(draft, dc, weights=wd), j)
-            # verify: next_ids and the k proposals at positions + 0..k, appended at rows [kv_end - 1, kv_end + k)
-            torch.add(tc.kv_end, k, out=end)
-            x = _block_step(model, tc, w, torch.cat([tc.next_ids[:, None], drafts], 1), tc.positions[:, None] + ar,
-                            end, ws, S_gen)
-            ops.verify_select(_logits_last(w, x), drafts, tc.history, tc.kv_end, tc.positions, tc.next_ids,
-                              tc.finished, limit, penalty, ngram, eos, pad, picks=picks)
+        def verify(logits):
+            ops.verify_select(logits, drafts, tc.history, tc.kv_end, tc.positions, tc.next_ids, tc.finished, limit,
+                              penalty, ngram, eos, pad, picks=picks)
 
-        step = _captured(round_, input_ids.is_cuda)
+        rnd = _SpecRound(model, draft, tc, dc, w, wd, k, S_gen, draft_select, verify)
+        drafts = rnd.drafts
+        step = _captured(rnd, input_ids.is_cuda)
         if max_new == 1:
             _host_sync([tc.finished.min()], *flags)
         else:
@@ -578,7 +607,7 @@ def _admit(model, cache: B200KVCache, limit: torch.Tensor, w: _Weights, batch, p
     attention_mask values (padding included: never attended by the new tokens), relabelled o_j + run index so the row's
     ids are non-decreasing and non-zero; the gap rows after it continue its last document (ids pad, features zero),
     so every 128-row q block holds rows of one prompt and sees the K/V blocks it sees when prefilled alone.  Slots not
-    in `batch` are not touched."""
+    in `batch` are not touched.  select=None (a draft model's cache) fills the cache and the state only: no lm_head."""
     lm, audio = _parts(model)
     dev = cache.data.device
     offs, o = [], 0
@@ -617,8 +646,9 @@ def _admit(model, cache: B200KVCache, limit: torch.Tensor, w: _Weights, batch, p
         return ops.attn_fwd(q, k, v, plan, cache.H, cache.KV, cache.scale)
 
     x = _layers(cache, w, x, cos, sin, attend)
-    last = torch.tensor([o0 + p.T - 1 for (_, p), o0 in zip(batch, offs)], dtype=torch.int64).to(dev)
-    select(_logits_last(w, x.index_select(0, last)), [slot for slot, _ in batch])
+    if select is not None:
+        last = torch.tensor([o0 + p.T - 1 for (_, p), o0 in zip(batch, offs)], dtype=torch.int64).to(dev)
+        select(_logits_last(w, x.index_select(0, last)), [slot for slot, _ in batch])
 
 
 def _sampling_args(temperature, top_k, top_p):
@@ -638,7 +668,8 @@ def _sampling_args(temperature, top_k, top_p):
 
 def generate_many(model, prompts, *, batch_size, max_new_tokens, eos_token_id, pad_token_id, repetition_penalty=1.0,
                   no_repeat_ngram_size=0, max_prompt_length=None, cuda_graph: bool = True, stats: Optional[dict] = None,
-                  do_sample: bool = False, temperature=None, top_k=None, top_p=None):
+                  do_sample: bool = False, temperature=None, top_k=None, top_p=None, assistant_model=None,
+                  num_assistant_tokens=None, num_assistant_tokens_schedule=None, **kwargs):
     """Greedy decoding, or multinomial sampling, of many prompts with continuous batching: a cache of `batch_size`
     slots; when a slot's row finishes (eos or its token budget), its generated ids are copied out and the next prompt is
     prefilled into that slot while the other slots keep decoding.  Per prompt, the greedy result is what `generate`
@@ -657,7 +688,16 @@ def generate_many(model, prompts, *, batch_size, max_new_tokens, eos_token_id, p
     max_prompt_length  the longest prompt to expect (default: the longest of `prompts` when it is a sequence)
     cuda_graph       False runs every decode step eagerly (the captured step computes the same bits)
     stats            if a dict, receives decode_steps, admissions and, on CUDA, admission_events (pairs of CUDA events
-                     around each admission prefill)"""
+                     around each admission prefill); with a draft also rounds (= decode_steps) and live_row_rounds
+                     (summed over rounds: the slots holding a prompt in that round)
+
+    assistant_model (HF's assisted generation, with num_assistant_tokens k and the checks of `generate`): speculative
+    decoding.  Each slot's prompt is prefilled into the same slot of a draft cache; per round the draft proposes k
+    tokens per slot and the model scores them in one step of B*(k+1) rows (_SpecRound).  Greedy: the result is the one
+    without the draft, bit for bit (tn_verify_select_bf16).  do_sample=True: speculative sampling
+    (tn_spec_sample_verify_bf16): the draft draws its proposals with tn_sample_select_slots_bf16 and the same knobs from
+    its own Philox streams (a second 64-bit seed, the next draw from torch's default CPU generator), and each prompt's
+    ids have exactly the distribution of sampling without the draft; its first token is the same draw."""
     budgets = None
     if isinstance(max_new_tokens, (list, tuple)) or (torch.is_tensor(max_new_tokens) and max_new_tokens.dim() == 1):
         budgets = [int(b) for b in max_new_tokens]
@@ -669,7 +709,15 @@ def generate_many(model, prompts, *, batch_size, max_new_tokens, eos_token_id, p
         max_budget = max(budgets)
     else:
         max_budget = int(max_new_tokens)
-    _validate(max_budget, eos_token_id, pad_token_id, repetition_penalty, no_repeat_ngram_size, False, 1, {})
+    draft, k = assistant_model, None
+    if draft is not None:
+        k = _spec_args(model, draft, num_assistant_tokens, num_assistant_tokens_schedule, kwargs)
+    elif kwargs:        # the keyword arguments of assisted generation only
+        raise TypeError(f"generate_many() got an unexpected keyword argument {next(iter(kwargs))!r}")
+    else:               # without a draft the assisted-generation knobs are unsupported arguments, as in `generate`
+        kwargs = dict(num_assistant_tokens=num_assistant_tokens,
+                      num_assistant_tokens_schedule=num_assistant_tokens_schedule)
+    _validate(max_budget, eos_token_id, pad_token_id, repetition_penalty, no_repeat_ngram_size, False, 1, kwargs)
     if do_sample:
         temperature, top_k, top_p = _sampling_args(temperature, top_k, top_p)
     _check_scope(model)
@@ -691,6 +739,7 @@ def generate_many(model, prompts, *, batch_size, max_new_tokens, eos_token_id, p
     if max_len < 1:
         raise TouchNetB200Error(f"generate_many: max_prompt_length must be >= 1, got {max_prompt_length}")
     eos, pad = int(eos_token_id), int(pad_token_id)
+    penalty, ngram = float(repetition_penalty), int(no_repeat_ngram_size)
     lm, audio = _parts(model)
     dev = lm.lm_head.weight.device
     it = iter(prompts)
@@ -699,7 +748,9 @@ def generate_many(model, prompts, *, batch_size, max_new_tokens, eos_token_id, p
     count = 0
     with torch.no_grad():
         w = _Weights(lm)
-        cache = B200KVCache(model, B, max_len + max_budget, device=dev)
+        S_gen = max_len + max_budget
+        # with a draft the verify step writes up to k rows past a slot's limit
+        cache = B200KVCache(model, B, S_gen if draft is None else S_gen + k, device=dev)
         limit = torch.zeros(B, dtype=torch.int32, device=dev)
         stream_key = torch.zeros(B, dtype=torch.int64, device=dev)    # the index of the prompt in each slot
         seed = int(torch.randint(-2**63, 2**63 - 1, (), dtype=torch.int64)) if do_sample else 0
@@ -719,6 +770,41 @@ def generate_many(model, prompts, *, batch_size, max_new_tokens, eos_token_id, p
                 ops.greedy_select_slots(logits, cache.history, cache.kv_end, cache.positions, cache.next_ids,
                                         cache.finished, limit, float(repetition_penalty), int(no_repeat_ngram_size),
                                         eos, pad, row_slot=slots)
+
+        if draft is None:
+            flags = (nan_flag,)
+            step = _captured(lambda: select(decode_step(model, cache, weights=w)), cuda_graph and dev.type == "cuda")
+        else:
+            dlm, daudio = _parts(draft)
+            wd = _Weights(dlm)
+            dc = B200KVCache(draft, B, S_gen + k, device=dev)
+            flags = (nan_flag, None if daudio is None else daudio._nan_flag)
+            dseed = int(torch.randint(-2**63, 2**63 - 1, (), dtype=torch.int64)) if do_sample else 0
+            dkey = torch.zeros(B, dtype=torch.int64, device=dev)
+            dlogits = torch.empty((B, k, cache.vocab), dtype=BF16, device=dev) if do_sample else None
+            picks = torch.zeros((B, k + 1), dtype=torch.int64, device=dev)
+
+            def draft_select(logits, j):
+                if do_sample:
+                    dlogits[:, j].copy_(logits)
+                    ops.sample_select_slots(logits, dc.history, dc.kv_end, dc.positions, dc.next_ids, dc.finished,
+                                            limit, dkey, penalty, ngram, temperature, top_k, top_p, dseed, eos, pad)
+                else:
+                    ops.greedy_select_slots(logits, dc.history, dc.kv_end, dc.positions, dc.next_ids, dc.finished,
+                                            limit, penalty, ngram, eos, pad)
+
+            def verify(logits):
+                if do_sample:
+                    ops.spec_sample_verify(logits, dlogits.view(B * k, -1), rnd.drafts, cache.history, cache.kv_end,
+                                           cache.positions, cache.next_ids, cache.finished, limit, stream_key, penalty,
+                                           ngram, temperature, top_k, top_p, seed, eos, pad, picks=picks)
+                else:
+                    ops.verify_select(logits, rnd.drafts, cache.history, cache.kv_end, cache.positions, cache.next_ids,
+                                      cache.finished, limit, penalty, ngram, eos, pad, picks=picks)
+
+            rnd = _SpecRound(model, draft, cache, dc, w, wd, k, S_gen, draft_select, verify,
+                             copies=((dkey, stream_key),) if do_sample else ())
+            step = _captured(rnd, cuda_graph and dev.type == "cuda")
 
         def admit(free) -> None:
             nonlocal count, admissions
@@ -742,18 +828,20 @@ def generate_many(model, prompts, *, batch_size, max_new_tokens, eos_token_id, p
                     ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
                     ev[0].record()
                 _admit(model, cache, limit, w, chunk, pad, select)
+                if draft is not None:             # the same slots of the draft's cache, no first-token selection
+                    _admit(draft, dc, limit, wd, chunk, pad, None)
                 admissions += 1
                 if ev is not None:
                     ev[1].record()
                     admission_events.append(ev)
 
-        step = _captured(lambda: select(decode_step(model, cache, weights=w)), cuda_graph and dev.type == "cuda")
         admit(list(range(B)))
-        steps = 0
+        steps = live_row_rounds = 0
         while any(p is not None for p in slot_prompt):
+            live_row_rounds += sum(p is not None for p in slot_prompt)
             step()
             steps += 1
-            vals = _host_sync([cache.finished, cache.kv_end], nan_flag)
+            vals = _host_sync([cache.finished, cache.kv_end], *flags)
             free = []
             for s in range(B):
                 p = slot_prompt[s]
@@ -765,6 +853,8 @@ def generate_many(model, prompts, *, batch_size, max_new_tokens, eos_token_id, p
                 admit(free)
         if stats is not None:
             stats.update(decode_steps=steps, admissions=admissions, admission_events=admission_events)
+            if draft is not None:
+                stats.update(rounds=steps, live_row_rounds=live_row_rounds)
     if budgets is not None and count != len(budgets):
         raise TouchNetB200Error(f"generate_many: {len(budgets)} budgets for {count} prompts")
     return [results[i] for i in range(count)]

@@ -791,6 +791,29 @@ def verify_select(logits, draft, history, length, positions, next_ids, finished,
     return picks
 
 
+def spec_sample_verify(logits, draft_logits, draft, history, length, positions, next_ids, finished, limit, stream_key,
+                       repetition_penalty: float, no_repeat_ngram_size: int, temperature: float, top_k: int,
+                       top_p: float, seed: int, eos: int, pad: int, picks=None):
+    """Speculative sampling over logits [B*(k+1), V], the draft's logits draft_logits [B*k, V] and its tokens draft
+    [B, k] (see tn_spec_sample_verify_bf16): each draft token is accepted with probability min(1, p/q), the first
+    rejection emits a token of the residual max(0, p - q) (all accepted: one of p_k), and the emitted tokens are
+    committed as verify_select commits its picks.  Returns picks [B, k+1] (x accepted, ~t emitted; rows not finished)."""
+    n, V = _select_dims(logits, history, length, positions, next_ids, finished)
+    _chk(draft_logits, "draft_logits", BF16); _chk(draft, "draft", torch.int64); _chk(limit, "limit", torch.int32)
+    _chk(stream_key, "stream_key", torch.int64)
+    B, k = draft.shape
+    assert n == B * (k + 1) and tuple(draft_logits.shape) == (B * k, V) and draft_logits.stride(1) == 1
+    assert history.shape[0] == B and draft.is_contiguous()
+    if picks is None:
+        picks = torch.empty((B, k + 1), dtype=torch.int64, device=logits.device)
+    _lib.call("tn_spec_sample_verify_bf16", logits.data_ptr(), logits.stride(0), draft_logits.data_ptr(),
+              draft_logits.stride(0), B, k, V, draft.data_ptr(), history.data_ptr(), history.stride(0),
+              length.data_ptr(), positions.data_ptr(), next_ids.data_ptr(), finished.data_ptr(), limit.data_ptr(),
+              stream_key.data_ptr(), picks.data_ptr(), float(repetition_penalty), int(no_repeat_ngram_size),
+              float(temperature), int(top_k), float(top_p), int(seed), int(eos), int(pad), _st())
+    return picks
+
+
 def _host_i32(rows) -> torch.Tensor:
     """A small int32 table in host memory (the continuous-batching entry points copy it into the launch)."""
     return torch.tensor(rows, dtype=torch.int32).reshape(-1).contiguous()
