@@ -143,6 +143,17 @@ int tn_gemm_qkv_fp8_rowwise(int mode, const void* A, int64_t lda, const void* B0
                             int M, int N, int K, const void* rope_cos, const void* rope_sin, const float* inv_sa,
                             const float* inv_sb, tn_stream_t stream);
 
+/* Skinny-M rowwise FP8 GEMM for cached decode steps: D[M,N] = X[M,K]·Wᵀ with X bf16 and W e4m3 rows as
+ * tn_fp8_rowwise_cast_bf16 writes them (inv_sw their 1/s).  The kernel quantises each row of X with that cast's rule (the
+ * same power-of-two scale and sat_rne bytes) and accumulates over K in a fixed order, so each element of D depends only
+ * on its row of X, W, inv_sw and R[m,n]: not on M, the row's position or the other rows.  Epilogues in the rounding
+ * order of the rowwise wgmma GEMMs: epi 0 D = bf16(acc·1/s_x·1/s_w); epi 1 D = bf16(that + R) (R bf16 [M,N], ldr);
+ * epi 2 (SwiGLU) W = [Wg;Wu] (2N rows, inv_sw [2N] stacked the same way), D = H = silu(G)⊙U as
+ * tn_gemm_swiglu_fp8_rowwise computes it, G and U not stored.  Any M >= 1; N and K multiples of 16; ldw a multiple of
+ * 16.  Allocates nothing and never syncs the host (graph-capturable). */
+int tn_gemm_fp8_decode(const void* X, int64_t ldx, const void* W, int64_t ldw, const float* inv_sw, int epi,
+                       const void* R, int64_t ldr, void* D, int64_t ldd, int M, int N, int K, tn_stream_t stream);
+
 /* SwiGLU backward (elementwise): dG = dH⊙U⊙silu'(G), dU = dH⊙silu(G).  bf16 [M,N] contiguous rows (ld). */
 int tn_swiglu_bwd_bf16(const void* G, const void* U, const void* dH, void* dG, void* dU, int64_t rows, int64_t cols,
                        int64_t ld, tn_stream_t stream);

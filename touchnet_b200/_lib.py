@@ -44,6 +44,7 @@ _SIGNATURES = {
     "tn_gemm_dswiglu_fp8_rowwise": [_vp, _i64, _vp, _i64, _vp, _vp, _i64, _vp, _vp, _i64, _i, _i, _i, _vp, _vp, _vp],
     "tn_gemm_qkv_fp8_rowwise": [_i, _vp, _i64, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _i64, _i, _i, _i, _i, _i, _i, _i,
                                 _vp, _vp, _vp, _vp, _vp],
+    "tn_gemm_fp8_decode": [_vp, _i64, _vp, _i64, _vp, _i, _vp, _i64, _vp, _i64, _i, _i, _i, _vp],
     "tn_swiglu_bwd_bf16": [_vp, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _vp],
     "tn_rmsnorm_fwd_bf16": [_vp, _vp, _vp, _i, _vp, _vp, _vp, _i64, _i, _f, _vp],
     "tn_rmsnorm_bwd_bf16": [_vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _i, _vp, _i64, _i, _vp],

@@ -244,6 +244,196 @@ fp8_colwise_cast_t_kernel(const bf16* __restrict__ x, int64_t ldx, int64_t rows,
   *reinterpret_cast<uint4*>(out_t + c * ld_out_t + r) = make_uint4(w[0], w[1], w[2], w[3]);
 }
 
+// ------------------------------------------- skinny-M decode GEMM (rowwise e4m3) -------------------------------------------
+// D[M, N] = X[M, K]·W[N, K]ᵀ for the few rows of a cached decode step.  The weight is far too narrow in M for the wgmma
+// tiles, so the kernel streams W once per group of up to 64 rows of X:
+//   - each CTA quantises its group of X rows into shared memory with the rule of fp8_rowwise_cast_kernel (the same amax,
+//     power-of-two scale and sat_rne bytes; rows past M are zero), then loops over 8-column tiles of W (persistent grid);
+//   - within a tile the 8 warps split K: warp w takes the 64-byte chunks w, w + 8, ... and accumulates them in order with
+//     mma.sync.m16n8k32 e4m3 (16 rows of X per MMA).  Each lane loads one 16-byte piece of a weight row per chunk and
+//     feeds its halves to two MMAs; the X bytes are read from shared memory with the same permutation of k, so the sum
+//     is over the same products;
+//   - the 8 warp partials are added in warp order through shared memory, then the rowwise epilogue runs.
+// An output element depends on its row of X, W, inv_sw (and R) only: the MMA's rows are independent, the chunk order is a
+// function of K, and nothing is atomic.
+constexpr int kDecThreads = 256;
+constexpr int kDecWarps = kDecThreads / 32;
+constexpr int kDecTileN = 8;                    // output columns per tile (one n8 MMA)
+constexpr int kDecMaxMTiles = 4;                // 64 rows of X per group
+constexpr int kDecSmemMax = 200 * 1024;
+
+__device__ __forceinline__ void mma_e4m3_16832(float* c, uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3,
+                                               uint32_t b0, uint32_t b1) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k32.row.col.f32.e4m3.e4m3.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+      "{%0, %1, %2, %3};"
+      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+      : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
+}
+
+// shared-memory pitch of a quantised X row: holds K rounded up to 64 (zero tail), and is 64 mod 128 so that the two rows
+// each quarter-warp reads sit in different banks
+__host__ __device__ constexpr int dec_pitch(int K) { return (K + 127) / 128 * 128 + 64; }
+
+__host__ __device__ constexpr int dec_smem(int K, int mtiles, int nw) {
+  return mtiles * 16 * dec_pitch(K) + mtiles * 16 * 4 + kDecWarps * nw * mtiles * 16 * kDecTileN * 4;
+}
+
+// EPI 0: bf16(acc·ia·iw); 1: + R; 2: SwiGLU over W = [Wg; Wu] (2N rows), H only.  MT: 16-row MMA tiles per group.
+template <int EPI, int MT>
+__global__ void __launch_bounds__(kDecThreads)
+fp8_decode_gemm_kernel(const bf16* __restrict__ x, int64_t ldx, const uint8_t* __restrict__ w, int64_t ldw,
+                       const float* __restrict__ inv_sw, const bf16* __restrict__ r, int64_t ldr, bf16* __restrict__ d,
+                       int64_t ldd, int M, int N, int K) {
+  constexpr int NW = EPI == 2 ? 2 : 1;          // weight rows per output column
+  constexpr int G = 16 * MT;
+  constexpr int U = EPI == 2 && MT > 2 ? 2 : 8 / NW;   // chunks in flight per batch (no spill at 64 SwiGLU rows)
+  extern __shared__ __align__(16) uint8_t dsm[];
+  const int pitch = dec_pitch(K);
+  uint8_t* xq = dsm;
+  float* ia = reinterpret_cast<float*>(dsm + G * pitch);
+  float* red = ia + G;                          // [warp][NW][G][8]
+  const int warp = int(threadIdx.x) >> 5, lane = int(threadIdx.x) & 31;
+  const int g = lane >> 2, tig = lane & 3;
+  const int m0 = int(blockIdx.y) * G;
+  const int kpad = (K + 63) / 64 * 64, nch = kpad / 64, ntiles = N / kDecTileN;
+
+  // the first tile's weight lines start on their way to L2 while X is quantised
+  if (int(blockIdx.x) < ntiles)
+    for (int c = warp; c < nch; c += kDecWarps) {
+      const int k = 64 * c + 16 * tig;
+      if (k < K)
+#pragma unroll
+        for (int j = 0; j < NW; ++j)
+          asm volatile("prefetch.global.L2 [%0];" ::"l"(w + (int64_t(j) * N + kDecTileN * blockIdx.x + g) * ldw + k));
+    }
+
+  // X rows -> e4m3 in shared memory, one warp per row (fp8_rowwise_cast_kernel's amax, scale and bytes)
+  for (int rr = warp; rr < G; rr += kDecWarps) {
+    uint8_t* q = xq + rr * pitch;
+    const int row = m0 + rr;
+    if (row < M) {
+      const bf16* xr = x + int64_t(row) * ldx;
+      uint32_t m = 0;
+      for (int ch = lane; ch < K / 8; ch += 32) m = max(m, absmax8(__ldg(reinterpret_cast<const uint4*>(xr + 8 * ch))));
+      m = __reduce_max_sync(0xffffffffu, m);
+      const float s = fp8_pow2_scale(__uint_as_float(m));
+      if (lane == 0) ia[rr] = __frcp_rn(s);
+      for (int ch = lane; ch < K / 8; ch += 32)
+        *reinterpret_cast<uint2*>(q + 8 * ch) =
+            cast8_e4m3(__ldg(reinterpret_cast<const uint4*>(xr + 8 * ch)), s, s, s, s, s, s, s, s);
+      for (int ch = K / 8 + lane; ch < kpad / 8; ch += 32) *reinterpret_cast<uint2*>(q + 8 * ch) = make_uint2(0, 0);
+    } else {
+      if (lane == 0) ia[rr] = 0.f;
+      for (int ch = lane; ch < kpad / 8; ch += 32) *reinterpret_cast<uint2*>(q + 8 * ch) = make_uint2(0, 0);
+    }
+  }
+  __syncthreads();
+
+  for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
+    const int n0 = kDecTileN * t;
+    float acc[NW][MT][4];
+#pragma unroll
+    for (int j = 0; j < NW; ++j)
+#pragma unroll
+      for (int i = 0; i < MT; ++i) acc[j][i][0] = acc[j][i][1] = acc[j][i][2] = acc[j][i][3] = 0.f;
+    const uint8_t* wr[NW];
+#pragma unroll
+    for (int j = 0; j < NW; ++j) wr[j] = w + (int64_t(j) * N + n0 + g) * ldw + 16 * tig;
+    for (int c0 = warp; c0 < nch; c0 += kDecWarps * U) {
+      uint4 b[U][NW];
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+        const int c = c0 + kDecWarps * u;
+        const bool ok = c < nch && 64 * c + 16 * tig < K;   // K % 16 == 0: a piece is wholly inside or outside
+#pragma unroll
+        for (int j = 0; j < NW; ++j)
+          b[u][j] = ok ? __ldg(reinterpret_cast<const uint4*>(wr[j] + 64 * c)) : make_uint4(0, 0, 0, 0);
+      }
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+        const int c = c0 + kDecWarps * u;
+        if (c >= nch) break;                                 // warp-uniform
+        const uint8_t* qa = xq + g * pitch + 64 * c + 16 * tig;
+#pragma unroll
+        for (int i = 0; i < MT; ++i) {
+          const uint4 lo = *reinterpret_cast<const uint4*>(qa + 16 * i * pitch);
+          const uint4 hi = *reinterpret_cast<const uint4*>(qa + (16 * i + 8) * pitch);
+#pragma unroll
+          for (int j = 0; j < NW; ++j) {
+            mma_e4m3_16832(acc[j][i], lo.x, hi.x, lo.y, hi.y, b[u][j].x, b[u][j].y);
+            mma_e4m3_16832(acc[j][i], lo.z, hi.z, lo.w, hi.w, b[u][j].z, b[u][j].w);
+          }
+        }
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < NW; ++j)
+#pragma unroll
+      for (int i = 0; i < MT; ++i) {
+        float* p = red + ((warp * NW + j) * G + 16 * i + g) * kDecTileN + 2 * tig;
+        *reinterpret_cast<float2*>(p) = make_float2(acc[j][i][0], acc[j][i][1]);
+        *reinterpret_cast<float2*>(p + 8 * kDecTileN) = make_float2(acc[j][i][2], acc[j][i][3]);
+      }
+    __syncthreads();
+    for (int e = int(threadIdx.x); e < G * kDecTileN; e += kDecThreads) {
+      const int rr = e / kDecTileN, row = m0 + rr, col = n0 + e % kDecTileN;
+      if (row >= M) continue;
+      float s[NW];
+#pragma unroll
+      for (int j = 0; j < NW; ++j) {
+        s[j] = red[j * G * kDecTileN + e];
+#pragma unroll
+        for (int v = 1; v < kDecWarps; ++v) s[j] += red[(v * NW + j) * G * kDecTileN + e];
+      }
+      // the rowwise wgmma epilogue's order: (acc · 1/s_a) · 1/s_b, rounded to bf16
+      float out;
+      if constexpr (EPI == 2) {
+        const float gt = bf16_round(s[0] * ia[rr] * inv_sw[col]);
+        const float up = bf16_round(s[1] * ia[rr] * inv_sw[N + col]);
+        out = bf16_round(gt / (1.f + __expf(-gt))) * up;
+      } else {
+        out = s[0] * ia[rr] * inv_sw[col];
+        if constexpr (EPI == 1) out = bf16_round(out) + __bfloat162float(r[int64_t(row) * ldr + col]);
+      }
+      d[int64_t(row) * ldd + col] = __float2bfloat16_rn(out);
+    }
+    __syncthreads();
+  }
+}
+
+template <int EPI, int MT>
+static int launch_decode_gemm(const bf16* x, int64_t ldx, const uint8_t* w, int64_t ldw, const float* inv_sw,
+                              const bf16* r, int64_t ldr, bf16* d, int64_t ldd, int M, int N, int K,
+                              cudaStream_t stream) {
+  auto kern = fp8_decode_gemm_kernel<EPI, MT>;
+  static bool attr = false;
+  if (!attr) {
+    TN_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kDecSmemMax));
+    attr = true;
+  }
+  const int smem = dec_smem(K, MT, EPI == 2 ? 2 : 1);
+  int per_sm = 0;
+  TN_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kDecThreads, smem));
+  const int groups = (M + 16 * MT - 1) / (16 * MT), ntiles = N / kDecTileN;
+  const int ctas = max(1, max(per_sm, 1) * sm_count() / groups);
+  const dim3 grid(unsigned(min(ntiles, ctas)), unsigned(groups));
+  kern<<<grid, kDecThreads, smem, stream>>>(x, ldx, w, ldw, inv_sw, r, ldr, d, ldd, M, N, K);
+  TN_CHECK_CUDA(cudaGetLastError());
+  return TN_OK;
+}
+
+template <int EPI>
+static int decode_gemm(int mt, const bf16* x, int64_t ldx, const uint8_t* w, int64_t ldw, const float* inv_sw,
+                       const bf16* r, int64_t ldr, bf16* d, int64_t ldd, int M, int N, int K, cudaStream_t stream) {
+  switch (mt) {
+    case 1: return launch_decode_gemm<EPI, 1>(x, ldx, w, ldw, inv_sw, r, ldr, d, ldd, M, N, K, stream);
+    case 2: return launch_decode_gemm<EPI, 2>(x, ldx, w, ldw, inv_sw, r, ldr, d, ldd, M, N, K, stream);
+    case 3: return launch_decode_gemm<EPI, 3>(x, ldx, w, ldw, inv_sw, r, ldr, d, ldd, M, N, K, stream);
+    default: return launch_decode_gemm<EPI, 4>(x, ldx, w, ldw, inv_sw, r, ldr, d, ldd, M, N, K, stream);
+  }
+}
+
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 static bool aligned4(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) == 0; }
 
@@ -338,3 +528,33 @@ extern "C" int tn_fp8_colwise_cast_t_bf16(const void* x, int64_t ldx, int64_t ro
   return TN_OK;
 }
 #undef TN_AXIS_REQUIRE_X
+
+extern "C" int tn_gemm_fp8_decode(const void* X, int64_t ldx, const void* W, int64_t ldw, const float* inv_sw, int epi,
+                                  const void* R, int64_t ldr, void* D, int64_t ldd, int M, int N, int K,
+                                  tn_stream_t stream_) {
+  clear_error();
+  TN_REQUIRE(X && W && inv_sw && D, "tn_gemm_fp8_decode: null pointer (X, W, inv_sw and D)");
+  TN_REQUIRE(epi >= 0 && epi <= 2, "tn_gemm_fp8_decode: epi=%d must be 0 (plain), 1 (+ residual) or 2 (SwiGLU)", epi);
+  TN_REQUIRE((epi == 1) == (R != nullptr), "tn_gemm_fp8_decode: R is required with epi 1 and only there");
+  TN_REQUIRE(M > 0 && N > 0 && K > 0 && N % 16 == 0 && K % 16 == 0,
+             "tn_gemm_fp8_decode: M=%d must be positive, N=%d and K=%d positive multiples of 16", M, N, K);
+  TN_REQUIRE(dec_smem(K, 1, epi == 2 ? 2 : 1) <= kDecSmemMax, "tn_gemm_fp8_decode: K=%d too large (16 rows of X must "
+             "fit in shared memory)", K);
+  TN_REQUIRE(ldx >= K && ldx % 8 == 0 && aligned16(X), "tn_gemm_fp8_decode: X must be 16 B aligned with ldx >= K, a "
+             "multiple of 8");
+  TN_REQUIRE(ldw >= K && ldw % 16 == 0 && aligned16(W), "tn_gemm_fp8_decode: W must be 16 B aligned with ldw >= K, a "
+             "multiple of 16");
+  TN_REQUIRE(aligned4(inv_sw), "tn_gemm_fp8_decode: inv_sw must be 4 B aligned");
+  TN_REQUIRE(ldd >= N && (!R || ldr >= N), "tn_gemm_fp8_decode: ldd and ldr must be >= N");
+  const int need = (M + 15) / 16;
+  int mt = need < kDecMaxMTiles ? need : kDecMaxMTiles;
+  while (mt > 1 && dec_smem(K, mt, epi == 2 ? 2 : 1) > kDecSmemMax) --mt;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  const bf16* x = static_cast<const bf16*>(X);
+  const uint8_t* w = static_cast<const uint8_t*>(W);
+  const bf16* r = static_cast<const bf16*>(R);
+  bf16* d = static_cast<bf16*>(D);
+  if (epi == 0) return decode_gemm<0>(mt, x, ldx, w, ldw, inv_sw, r, ldr, d, ldd, M, N, K, stream);
+  if (epi == 1) return decode_gemm<1>(mt, x, ldx, w, ldw, inv_sw, r, ldr, d, ldd, M, N, K, stream);
+  return decode_gemm<2>(mt, x, ldx, w, ldw, inv_sw, r, ldr, d, ldd, M, N, K, stream);
+}

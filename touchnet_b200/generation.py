@@ -124,6 +124,11 @@ class _Weights:
             inv, _ = rot.rope_init_fn(rot.config, device=inv.device)
         self.inv_freq = inv.detach().float().contiguous()
         self.rope_scaling = float(rot.attention_scaling)
+        # float8_inference: e4m3 copies of every block's projections (ops.float8_inference_weights), or None
+        self.float8 = None
+        if lm.float8_inference:
+            self.float8 = [ops.float8_inference_weights(lw[1], lw[2], lw[3], lw[7], lw[9], lw[10], lw[11])
+                        for lw in self.layers]
 
 
 def _check_scope(model) -> None:
@@ -184,15 +189,31 @@ def _prompt_front(model, w: _Weights, input_ids, input_features, doc, pos):
     return (x, ops.AttnPlan(doc), *ops.rope_table(pos, w.inv_freq, w.rope_scaling))
 
 
-def _layers(cache: B200KVCache, w: _Weights, x, cos, sin, attend, qkv_rows=None):
+def _pad_rows(t: torch.Tensor, rows: int) -> torch.Tensor:
+    return t if t.shape[0] == rows else torch.cat([t, t.new_zeros((rows - t.shape[0], *t.shape[1:]))])
+
+
+def _layers(cache: B200KVCache, w: _Weights, x, cos, sin, attend, qkv_rows=None, step: bool = False):
     """Every block over the rows x; `attend(q, k, v, k_cache, v_cache) -> (o, lse)` stores the layer's K/V into its
-    cache and runs the attention.  `qkv_rows`: see ops.block_forward."""
+    cache and runs the attention.  `qkv_rows`: see ops.block_forward.  `step`: a cached step (decode, draft or verify)
+    rather than a prompt pass; with FP8 weights (w.float8) it selects the kernels (ops.RowwiseInference), and a prompt
+    pass runs on its rows zero-padded to a multiple of 16 (row scales keep the padding out of the real rows)."""
+    M = x.shape[0]
+    Mp = M if w.float8 is None or step else -(-M // 16) * 16
+    if Mp != M:
+        x, cos, sin = _pad_rows(x, Mp), _pad_rows(cos, Mp), _pad_rows(sin, Mp)
+        inner = attend
+
+        def attend(q, k, v, kc, vc):
+            o, lse = inner(q[:M], k[:M], v[:M], kc, vc)
+            return _pad_rows(o, Mp), lse
+
     for i, lw in enumerate(w.layers):
         kc, vc = cache.layer(i)
-        x, _ = ops.block_forward(x, *lw, cos, sin, cache.H, cache.KV, w.eps, cache.hd,
-                                 lambda q, k, v, kc=kc, vc=vc: (*attend(q, k, v, kc, vc), k, v), need_gu=False,
-                                 qkv_rows=qkv_rows)
-    return x
+        x, _ = ops.cached_block_forward(x, lw, cos, sin, cache.H, cache.KV, w.eps, cache.hd,
+                                        lambda q, k, v, kc=kc, vc=vc: (*attend(q, k, v, kc, vc), k, v),
+                                        qkv_rows=qkv_rows, float8=None if w.float8 is None else w.float8[i], step=step)
+    return x[:M] if Mp != M else x
 
 
 def prefill(model, cache: B200KVCache, input_ids, input_features=None, attention_mask=None, position_ids=None,
@@ -239,7 +260,7 @@ def decode_step(model, cache: B200KVCache, weights: Optional[_Weights] = None) -
         o = ops.attn_decode(q, kc, vc, cache.kv_start, cache.kv_end, cache.H, cache.KV, cache.scale, cache.workspace)
         return o, None
 
-    return _logits_last(w, _layers(cache, w, x, cos, sin, attend))
+    return _logits_last(w, _layers(cache, w, x, cos, sin, attend, step=True))
 
 
 def forward_cached(model, cache: B200KVCache, input_ids, input_features=None, attention_mask=None, position_ids=None):
@@ -434,7 +455,7 @@ def _block_step(model, cache: B200KVCache, w: _Weights, ids, pos, end, workspace
         return ops.attn_decode_multi(q, kc[:, :s_attn], vc[:, :s_attn], cache.kv_start, end, Tq, cache.H, cache.KV,
                                      cache.scale, workspace), None
 
-    return _layers(cache, w, x, cos, sin, attend, qkv_rows=B)
+    return _layers(cache, w, x, cos, sin, attend, qkv_rows=B, step=True)
 
 
 def _multi_ws(cache: B200KVCache, Tq: int, s_attn: int) -> torch.Tensor:

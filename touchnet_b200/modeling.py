@@ -183,9 +183,11 @@ class B200LlamaModel(nn.Module):
         self.layers = nn.ModuleList([B200DecoderLayer(config, i) for i in range(config.num_hidden_layers)])
         self.norm = B200RMSNorm(config.hidden_size, _cfg(config, "rms_norm_eps", 1e-6))
         self.rotary_emb = B200RotaryEmbedding(config)
-        # FP8 projections in every decoder block (ops.block_forward); cached decoding stays bf16.  A plain attribute:
-        # no parameter or buffer, so state dicts do not change
+        # FP8 projections in every decoder block (ops.block_forward); cached decoding follows float8_inference, not
+        # this.  Plain attributes: no parameter or buffer, so state dicts do not change
         self.float8_training = bool(_cfg(config, "float8_training", False))
+        # FP8 (rowwise e4m3) projections in cached decoding: prefill, decode, speculative and generate_many steps
+        self.float8_inference = bool(_cfg(config, "float8_inference", False))
         # the FP8 recipe when float8_training is on: "tensorwise" (default) or "rowwise"
         self.float8_recipe_name = ops.check_fp8_recipe(_cfg(config, "float8_recipe_name", "tensorwise"))
         hd = _cfg(config, "head_dim", config.hidden_size // config.num_attention_heads)
@@ -297,7 +299,7 @@ class B200LlamaForCausalLM(nn.Module):
     def __init__(self, config):
         super().__init__()
         self.config = config
-        self.model = B200LlamaModel(config)       # reads the config key `float8_training`
+        self.model = B200LlamaModel(config)       # reads the config keys `float8_training`, `float8_inference`
         self.vocab_size = config.vocab_size
         self.lm_head = nn.Linear(config.hidden_size, config.vocab_size, bias=False)
         if _cfg(config, "tie_word_embeddings", False):
@@ -308,12 +310,27 @@ class B200LlamaForCausalLM(nn.Module):
     @property
     def float8_training(self) -> bool:
         """FP8 (torchao tensorwise recipe) for the q/k/v/o/gate/up/down projections of every decoder block, forward and
-        backward; lm_head, attention, norms and cached decoding stay bf16.  Set from the config key `float8_training`."""
+        backward; lm_head, attention and norms stay bf16, and cached decoding follows float8_inference.  Set from the config
+        key `float8_training`."""
         return self.model.float8_training
 
     @float8_training.setter
     def float8_training(self, v: bool):
         self.model.float8_training = bool(v)
+
+    @property
+    def float8_inference(self) -> bool:
+        """FP8 for the q/k/v/o/gate/up/down projections of cached decoding (prefill, decode_step, forward_cached,
+        generate, speculative decoding, generate_many), always with the rowwise recipe (one power-of-two scale per row,
+        so a row's result does not depend on the other rows): weights quantised once per call, the prompt through the
+        rowwise wgmma GEMMs, every cached step through tn_gemm_fp8_decode.  Embedding, norms, biases, the audio
+        projector, lm_head and the KV cache stay bf16, as does the uncached forward.  Set from the config key
+        `float8_inference`."""
+        return self.model.float8_inference
+
+    @float8_inference.setter
+    def float8_inference(self, v: bool):
+        self.model.float8_inference = bool(v)
 
     @property
     def float8_recipe_name(self) -> str:
@@ -456,6 +473,8 @@ class B200TouchAudioForCausalLM(nn.Module):
             self.float8_training = config.float8_training
         if getattr(config, "float8_recipe_name", None) is not None:
             self.float8_recipe_name = config.float8_recipe_name
+        if getattr(config, "float8_inference", None) is not None:
+            self.float8_inference = config.float8_inference
 
     @property
     def fused_linear_ce(self) -> bool:
@@ -472,6 +491,14 @@ class B200TouchAudioForCausalLM(nn.Module):
     @float8_training.setter
     def float8_training(self, v: bool):
         self.language_model.float8_training = bool(v)
+
+    @property
+    def float8_inference(self) -> bool:
+        return self.language_model.float8_inference
+
+    @float8_inference.setter
+    def float8_inference(self, v: bool):
+        self.language_model.float8_inference = bool(v)
 
     @property
     def float8_recipe_name(self) -> str:

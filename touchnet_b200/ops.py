@@ -544,6 +544,38 @@ def gemm_qkv_wgrad_fp8_rowwise(dqkv_t, x_t, f32: bool, nq: int, nkv: int, inv_a,
     return outs
 
 
+def gemm_fp8_decode(x, w8, inv_w, residual=None, swiglu: bool = False):
+    """The skinny-M rowwise GEMM of cached decode steps: bf16 x [M, K] (quantised row by row inside the kernel, with
+    fp8_rowwise_cast's rule) times e4m3 w8 [N, K] with 1/s inv_w [N]; returns bf16 [M, N], plus the bf16 `residual`
+    [M, N] if given.  swiglu=True: w8 = [Wg; Wu] [2N, K], inv_w [2N] stacked the same way, returns H = silu(G)⊙U [M, N].
+    Each output row depends on its row of x only.  Any M; N and K multiples of 16."""
+    _fp8_axis_input(x)
+    if w8.dtype != F8E4M3 or w8.dim() != 2 or w8.stride(1) != 1:
+        raise _lib.TouchNetB200Error(f"w8 must be a 2-D float8_e4m3fn view with unit inner stride, got {w8.dtype} "
+                                     f"{tuple(w8.shape)}")
+    (M, K), rows = x.shape, w8.shape[0]
+    if w8.shape[1] != K:
+        raise _lib.TouchNetB200Error(f"x {tuple(x.shape)} and w8 {tuple(w8.shape)} differ in K")
+    if swiglu and (residual is not None or rows % 2):
+        raise _lib.TouchNetB200Error("swiglu takes the stacked [Wg; Wu] (an even row count) and no residual")
+    N = rows // 2 if swiglu else rows
+    _fp8_vec(inv_w, rows, "inv_w")
+    if M < 1 or N % 16 or K % 16 or N == 0 or K == 0:
+        raise _lib.TouchNetB200Error(f"gemm_fp8_decode: N={N} and K={K} must be positive multiples of 16, M={M} >= 1")
+    out = torch.empty((M, N), dtype=BF16, device=x.device)
+    if residual is not None:
+        if residual.dtype != BF16 or tuple(residual.shape) != (M, N) or residual.stride(1) != 1:
+            raise _lib.TouchNetB200Error(f"residual must be bfloat16 {(M, N)} with unit inner stride, got "
+                                         f"{residual.dtype} {tuple(residual.shape)}")
+        _chk(residual, "residual")
+    for t, n in ((x, "x"), (w8, "w8"), (inv_w, "inv_w")):
+        _chk(t, n)
+    _lib.call("tn_gemm_fp8_decode", x.data_ptr(), x.stride(0), w8.data_ptr(), w8.stride(0), inv_w.data_ptr(),
+              2 if swiglu else int(residual is not None), _lib.ptr(residual),
+              0 if residual is None else residual.stride(0), out.data_ptr(), out.stride(0), M, N, K, _st())
+    return out
+
+
 def _fp8_quant(xs, st, slot: int, e5m2: bool, row: bool = True, t: bool = True):
     """Quantise the bf16 tensors `xs` with one dynamic scale, the amax over all of them, kept in row `slot` of the
     device scale table st [n, 2] = (amax, 1/s).  Returns [(row-major, transposed)] per tensor."""
@@ -553,11 +585,11 @@ def _fp8_quant(xs, st, slot: int, e5m2: bool, row: bool = True, t: bool = True):
     return [fp8_cast(x, amax, e5m2, row, t, inv=st[slot, 1]) for x in xs]
 
 
-def _fp8_dims(*dims):
+def _fp8_dims(*dims, key: str = "float8_training"):
     """Every GEMM dimension of the FP8 block (and the row count) is a multiple of 16: 16-byte 8-bit TMA rows."""
     bad = [int(v) for v in dims if int(v) % 16]
     if bad:
-        raise _lib.TouchNetB200Error(f"float8_training: GEMM dimensions must be multiples of 16, got {bad}")
+        raise _lib.TouchNetB200Error(f"{key}: GEMM dimensions must be multiples of 16, got {bad}")
 
 
 # forward scale-table rows of the FP8 block: (amax, 1/s) of each GEMM input
@@ -1047,7 +1079,8 @@ def block_forward(x2, ln1, wqb, wkb, wvb, bq, bk, bv, wob, ln2, wgb, wub, wdb, c
     fp8=True (training only, no tensor parallelism): the seven projections run as FP8 GEMMs on dynamically scaled e4m3
     copies of their inputs and weights; h1, h2 and hm in `saved` are then the transposed e4m3 copies the weight
     gradients need, and saved ends with (oᵀ in e4m3, the recipe's saved scales).  `fp8_recipe`: "tensorwise" (one
-    scale per tensor, e5m2 gradients) or "rowwise" (per-row power-of-two scales, e4m3 throughout)."""
+    scale per tensor, e5m2 gradients) or "rowwise" (per-row power-of-two scales, e4m3 throughout), or for cached FP8
+    inference a RowwiseInference object (nothing saved for a backward)."""
     if fp8:
         return _block_forward_fp8(x2, ln1, wqb, wkb, wvb, bq, bk, bv, wob, ln2, wgb, wub, wdb, cos, sin, H, KV, eps, hd,
                                   attend, fp8_recipe)
@@ -1110,6 +1143,12 @@ class _Tensorwise:
         self.fwd = torch.zeros((8, 2), dtype=torch.float32, device=dev) if saved is None else saved
         self.bwd = None if saved is None else torch.zeros((5, 2), dtype=torch.float32, device=dev)
         self.state = self.fwd
+
+    @staticmethod
+    def qkv_plan(M, nq, nkv, rope_ok):
+        """(one QKV launch, RoPE in its epilogue) for M rows; rope_ok: no q/k/v bias and head_dim 128."""
+        fused = qkv_fusable(M, nq, nkv)
+        return fused, fused and rope_ok
 
     def act(self, x, slot):
         """(row-major copy, 1/s, transposed copy, 1/s) of a forward activation."""
@@ -1189,6 +1228,8 @@ class _Rowwise:
         self.state = torch.empty(off, dtype=torch.float32, device=dev) if saved is None else saved
         self.promoted = saved is not None
 
+    qkv_plan = staticmethod(_Tensorwise.qkv_plan)
+
     def saved_inv(self, slot):
         off, n = self.t_off[slot]
         return self.state[off:off + n]
@@ -1254,21 +1295,90 @@ class _Rowwise:
 _FP8_RECIPE_CLASSES = {"tensorwise": _Tensorwise, "rowwise": _Rowwise}
 
 
+def cached_block_forward(x2, weights, cos, sin, H, KV, eps, hd, attend, qkv_rows=None, float8=None, step=False):
+    """One block of cached decoding (generation.py) on its bf16 working weights: block_forward without the tensors
+    a backward needs, or with `float8` (the block's float8_inference_weights) the FP8 block under RowwiseInference."""
+    if float8 is None:
+        return block_forward(x2, *weights, cos, sin, H, KV, eps, hd, attend, need_gu=False, qkv_rows=qkv_rows)
+    return _block_forward_fp8(x2, *weights, cos, sin, H, KV, eps, hd, attend, RowwiseInference(float8, step))
+
+
+def float8_inference_weights(wqb, wkb, wvb, wob, wgb, wub, wdb):
+    """The e4m3 copies of one block's projections for cached FP8 inference (the model config key `float8_inference`),
+    made once per generate call: {slot: (stacked rows, their 1/s, row count of each weight)} for [Wq;Wk;Wv], Wo,
+    [Wg;Wu] and Wd.  Row scales make the stacked copy equal to the copies of its parts."""
+    _fp8_dims(wqb.shape[1], wqb.shape[0], wkb.shape[0], wob.shape[1], wgb.shape[0], key="float8_inference")
+    out = {}
+    for slot, ws in ((_F8_WQKV, (wqb, wkb, wvb)), (_F8_WO, (wob,)), (_F8_WGU, (wgb, wub)), (_F8_WD, (wdb,))):
+        w = ws[0] if len(ws) == 1 else torch.cat(ws)
+        out[slot] = (*fp8_rowwise_cast(w), [t.shape[0] for t in ws])
+    return out
+
+
+class RowwiseInference:
+    """The rowwise recipe for cached decoding: weights from float8_inference_weights, activations as a row-scaled copy only
+    (nothing is saved for a backward).  A prompt pass (`step=False`: prefill, generate_many admissions; rows padded to a
+    multiple of 16 by the caller) runs the rowwise wgmma kernels as the rowwise training forward does; a cached step
+    (`step=True`: decode, draft and verify steps, any row count) runs tn_gemm_fp8_decode on the bf16 rows, which
+    quantises them with the same rule, so a row's result does not depend on the other rows of the step.  Always rowwise:
+    a per-tensor activation scale would tie each row to its neighbours (slots, draft rows)."""
+
+    state = None
+
+    def __init__(self, weights8, step: bool):
+        self.w8, self.step = weights8, step
+
+    def qkv_plan(self, M, nq, nkv, rope_ok):
+        """(one QKV launch, RoPE in its epilogue): a cached step runs one decode launch over [Wq;Wk;Wv]."""
+        return (True, False) if self.step else _Rowwise.qkv_plan(M, nq, nkv, rope_ok)
+
+    def act(self, x, slot):
+        return (x, None, None, None) if self.step else (*fp8_rowwise_cast(x), None, None)
+
+    def weights(self, ws, slot):
+        w8, inv, sizes = self.w8[slot]
+        parts, invs, off = [], [], 0
+        for n in sizes:
+            parts.append(w8[off:off + n])
+            invs.append(inv[off:off + n])
+            off += n
+        return parts, invs, inv
+
+    def gemm(self, a, b, inv_a, inv_b, residual=None):
+        if self.step:
+            return gemm_fp8_decode(a, b, inv_b, residual=residual)
+        return gemm_fp8_rowwise(a, b, inv_a, inv_b, promoted=False, residual=residual)
+
+    def swiglu(self, x, wg, wu, inv_x, inv_w):
+        if self.step:
+            return None, None, gemm_fp8_decode(x, self.w8[_F8_WGU][0], inv_w, swiglu=True)
+        return gemm_swiglu_fp8_rowwise(x, wg, wu, inv_x, inv_w, need_gu=False)
+
+    def qkv_fwd(self, x, wq, wk, wv, inv_x, inv_w, rope):
+        if self.step:
+            return gemm_fp8_decode(x, self.w8[_F8_WQKV][0], inv_w)
+        return gemm_qkv_fwd_fp8_rowwise(x, wq, wk, wv, inv_x, inv_w, rope=rope)
+
+
 def _fp8_recipe(name, dev, wqb, wob, wgb, saved=None):
     return _FP8_RECIPE_CLASSES[check_fp8_recipe(name)](dev, (wqb.shape[1], wob.shape[1], wgb.shape[0]), saved)
 
 
 def _block_forward_fp8(x2, ln1, wqb, wkb, wvb, bq, bk, bv, wob, ln2, wgb, wub, wdb, cos, sin, H, KV, eps, hd, attend,
                        recipe="tensorwise"):
-    """block_forward with FP8 projections (see there) under `recipe` (_Tensorwise, _Rowwise)."""
+    """block_forward with FP8 projections (see there) under `recipe`: a name (_Tensorwise, _Rowwise), or a recipe
+    object (RowwiseInference)."""
     nq, nkv, d, ffn = wqb.shape[0], wkb.shape[0], wqb.shape[1], wgb.shape[0]
-    _fp8_dims(x2.shape[0], d, nq, nkv, wob.shape[1], ffn)
-    rc = _fp8_recipe(recipe, x2.device, wqb, wob, wgb)
+    if isinstance(recipe, str):
+        _fp8_dims(x2.shape[0], d, nq, nkv, wob.shape[1], ffn)
+        rc = _fp8_recipe(recipe, x2.device, wqb, wob, wgb)
+    else:
+        rc = recipe
     h1, _, rstd1 = rmsnorm_fwd(x2, ln1, eps)
     h1_8, ih1, h1_t, _ = rc.act(h1, _F8_H1)
     wqkv8, iwqkv, iwqkv_all = rc.weights([wqb, wkb, wvb], _F8_WQKV)
-    rope_in_gemm = qkv_fusable(h1.shape[0], nq, nkv) and bq is None and hd == 128
-    if qkv_fusable(h1.shape[0], nq, nkv):
+    fused, rope_in_gemm = rc.qkv_plan(h1.shape[0], nq, nkv, bq is None and hd == 128)
+    if fused:
         qkv = rc.qkv_fwd(h1_8, *wqkv8, ih1, iwqkv_all, (cos, sin) if rope_in_gemm else None)
         q, k, v = qkv[:, :nq], qkv[:, nq:nq + nkv], qkv[:, nq + nkv:]
     else:
