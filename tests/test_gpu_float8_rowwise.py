@@ -52,7 +52,9 @@ def _operands(M, N, K, seed=0):
     g = torch.Generator(device=dev).manual_seed(seed)
     a = torch.randn(M, K, device=dev, generator=g).bfloat16()
     a[:, :K // 16] *= 10                          # columns of outliers: the row scales differ from the tensor's
-    b = (torch.randn(N, K, device=dev, generator=g) * 0.02).bfloat16()
+    # each B row its own power of two, so that the column scales of the product differ from each other
+    b = torch.randn(N, K, device=dev, generator=g) * 0.02
+    b = (b * torch.exp2(torch.randint(-3, 5, (N, 1), device=dev, generator=g).float())).bfloat16()
     a8, ia = ops.fp8_rowwise_cast(a)
     b8, ib = ops.fp8_rowwise_cast(b)
     return a8, b8, ia, ib

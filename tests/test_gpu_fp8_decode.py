@@ -32,8 +32,10 @@ def _operands(M, N, K, seed=0, rows=None):
     dev = require_cuda()
     g = torch.Generator(device=dev).manual_seed(seed)
     x = torch.randn(M, K, device=dev, generator=g).bfloat16()
-    x[:, :K // 16] *= 10                       # outlier columns: row scales differ from each other
-    w = (torch.randn(rows or N, K, device=dev, generator=g) * 0.02).bfloat16()
+    x[:, :K // 16] *= 10                       # outlier columns (they scale every row alike)
+    # each weight row its own power of two, so that the row scales differ from each other
+    w = torch.randn(rows or N, K, device=dev, generator=g) * 0.02
+    w = (w * torch.exp2(torch.randint(-3, 5, (w.shape[0], 1), device=dev, generator=g).float())).bfloat16()
     w8, iw = ops.fp8_rowwise_cast(w)
     return x, w8, iw
 
